@@ -1,13 +1,13 @@
 #!/usr/bin/env python
 """bench.py — training images/sec of the fused LoRA step (BASELINE.json metric; default = configs[1], Qwen-Image-Edit).
 
-    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl b200|reference] [--config NAME]
+    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl b200|reference] [--config NAME] [--dump-outputs DIR]
 
---config  qwen_edit (default, BASELINE configs[1]) : Qwen-Image-Edit LoRA r=16 bf16, 512x512, cached embeds, batch 4 / GPU
+--config  qwen_edit (default, BASELINE configs[1]) : Qwen-Image-Edit LoRA r=16 bf16, 512x512, cached embeds, batch 1 / GPU
           flux_kontext       (configs[2]) : FLUX-Kontext LoRA r=32 with the YAML target regex, 19+38 blocks, T=512, batch 2 / GPU
           qwen_plus_sharded  (configs[3]) : Qwen-Image-Edit-2509, target + 2 controls (3 x 1024 image tokens, frame offsets 0,1,2), T=448,
-                                            batch 4 / GPU, frozen block weights sharded 1/N per rank when N > 1
-          qwen_multires      (configs[4]) : Qwen-Image-Edit LoRA r=16, every batch mixes {320^2, 512^2, 640^2} samples (pad-to-max layout, block GEMMs on ragged row bands,
+                                            batch 1 / GPU, frozen block weights sharded 1/N per rank when N > 1
+          qwen_multires      (configs[4]) : Qwen-Image-Edit LoRA r=16, every batch mixes a 512^2 and a 320^2 sample (pad-to-max layout, block GEMMs on ragged row bands,
                                             AttentionMaskMseLoss), batch 4 / GPU
 
 b200 arm     : one "step" = noisy-input -> fused MMDiT forward -> flow-matching loss -> fused backward -> NCCL all-reduce of the flat
@@ -19,6 +19,10 @@ b200 arm     : one "step" = noisy-input -> fused MMDiT forward -> flow-matching 
 reference arm: the reference's eager PyTorch path restated in oracle/mmdit_oracle.py (diffusers/peft are not installable offline —
                DESIGN.md; the restatement is pinned to the reference's own code by tests/test_reference_goldens.py), on the host cores;
                a step is a bounded sample (full-width depth-1 and depth-2 models at B=1, fwd+loss+bwd) fitted linearly in depth.
+--dump-outputs DIR: after the timed steps, rank 0 writes what the last timed step computed as float32 / float64 .npy files: loss,
+               the noise prediction of the target tokens (padded to the longest sample of a
+               multi-resolution batch), the flat LoRA gradient and the updated LoRA parameters (fixed seeded samples of at most 4 Mi values
+               each).  Inputs and weights are seeded, so two builds run with the same arguments can be compared output for output.
 Prints ONE JSON line on rank 0.
 """
 import argparse
@@ -46,30 +50,33 @@ S_TOK = CFG["T"] + 2 * CFG["hw"] ** 2
 FLOP_PER_IMAGE = flop_per_image(CFG["layers"], S_TOK)
 
 CONFIGS = {
-    "qwen_edit": dict(model="qwen", blocks=60, T=352, imgs=[(1, 32, 32)] * 2, B=4, r=16, metric=METRIC,
+    # batch 1 / GPU: the 60-block model's 41 GB of bf16 weights plus the activations of a batch of 4 do not fit an 80 GB H100
+    "qwen_edit": dict(model="qwen", blocks=60, T=352, imgs=[(1, 32, 32)] * 2, B=1, r=16, metric=METRIC,
                       workload="Qwen-Image-Edit LoRA r=16 bf16 512x512 cached embeds, 60 blocks D=3072 H=24, S=352 txt + 2x1024 img tokens"),
     "flux_kontext": dict(model="flux", blocks=57, T=512, imgs=[(1, 32, 32)] * 2, B=2, r=32,
                          metric="training images/sec (FLUX-Kontext LoRA r=32 bf16, 512x512, cached embeds)",
                          workload="FLUX-Kontext LoRA r=32 (YAML target regex: every block Linear, AdaLN linears, x_embedder) bf16 512x512, "
                                   "19 double + 38 single blocks, S=512 txt + 2x1024 img tokens"),
-    "qwen_plus_sharded": dict(model="qwen", blocks=60, T=448, imgs=[(1, 32, 32)] * 3, B=4, r=16,
+    "qwen_plus_sharded": dict(model="qwen", blocks=60, T=448, imgs=[(1, 32, 32)] * 3, B=1, r=16,
                               metric="training images/sec (Qwen-Image-Edit-2509 LoRA r=16 bf16, target + 2 controls 512x512, cached embeds)",
                               workload="Qwen-Image-Edit-2509 (Plus) LoRA r=16 bf16, 3 images/sample with frame offsets 0,1,2, 60 blocks, "
                                        "S=448 txt + 3x1024 img tokens"),
-    "qwen_multires": dict(model="qwen", blocks=60, T=352, imgs=None, B=4, r=16,
-                          metric="training images/sec (Qwen-Image-Edit LoRA r=16 bf16, multi-resolution {320,512,640}^2, cached embeds)",
-                          workload="Qwen-Image-Edit LoRA r=16 bf16, every batch = one 640^2 + one 320^2 + two 512^2 samples (target+control, "
-                                   "pad-to-max: 3200 image tokens), AttentionMaskMseLoss, 60 blocks"),
+    # two samples of different resolution per batch: with the 41 GB of weights, larger mixed batches do not fit an 80 GB H100
+    "qwen_multires": dict(model="qwen", blocks=60, T=352, imgs=None, B=2, r=16,
+                          metric="training images/sec (Qwen-Image-Edit LoRA r=16 bf16, multi-resolution {320,512}^2, cached embeds)",
+                          workload="Qwen-Image-Edit LoRA r=16 bf16, every batch = one 512^2 + one 320^2 sample (target+control, "
+                                   "pad-to-max: 2048 image tokens), AttentionMaskMseLoss, 60 blocks"),
 }
-MULTIRES_HW = [40, 20, 32, 32]  # latent-patch side of the four samples of a batch (640, 320, 512, 512 px)
+MULTIRES_HW = [32, 20]  # latent-patch side of the two samples of a batch (512, 320 px)
 
 
 def peaks():
     p = os.path.join(ROOT, "MEASURED_PEAKS.json")
     if os.path.exists(p):
         d = json.load(open(p))
-        return d.get("bf16_tflops", 1590.0), d.get("bf16_tflops_sustained", 1400.0), "measured"
-    return 1590.0, 1400.0, "fallback"
+        if "bf16_tflops" in d:
+            return d["bf16_tflops"], d.get("bf16_tflops_sustained", d["bf16_tflops"]), "MEASURED_PEAKS.json bf16_tflops (burst; kernels timed alone, L2 flushed between launches)"
+    return 989.0, 989.0, "H100 SXM data sheet, dense bf16 (not measured)"
 
 
 class ClockSampler:
@@ -199,7 +206,26 @@ def run_reference(args):
     _emit(line)
 
 
-# ====================================================================================================== B200 arm
+# ====================================================================================================== fused (CUDA) arm
+DUMP_SAMPLE = 4 << 20  # values per dumped array: 4 arrays x 16 MB stay under 64 MB
+
+
+def dump_outputs(d, loss, m, B, n_target):
+    import numpy as np
+    import torch
+    os.makedirs(d, exist_ok=True)
+    np.save(os.path.join(d, "loss.npy"), np.array([float(loss.item())], dtype=np.float64))
+    g = torch.Generator().manual_seed(0)
+    params = torch.cat([p.detach().reshape(-1).float() for p in m._lora_params.values()])
+    pred = m._ws["pred"].view(B, -1, 64)[:, :n_target]  # the target tokens the loss sees (the control tokens are not dumped)
+    for name, t in (("pred", pred), ("lora_grad", m.G32), ("lora_params", params)):
+        flat = t.detach().reshape(-1)
+        if flat.numel() > DUMP_SAMPLE:
+            idx = torch.randint(0, flat.numel(), (DUMP_SAMPLE,), generator=g).sort().values
+            flat = flat[idx.to(flat.device)]
+        np.save(os.path.join(d, f"{name}.npy"), flat.float().cpu().numpy())
+
+
 def _init_weights(m, dev):
     import torch
     g = torch.Generator(device=dev).manual_seed(1234)
@@ -300,7 +326,7 @@ def kernel_rooflines(dev, B, T, Limg):
 
 def library_baseline(dev, cfg, budget_s=150.0):
     """What the reference itself would run on this GPU: its eager PyTorch step (oracle restatement: cuBLASLt bf16 GEMMs + SDPA, autograd,
-    clip, torch AdamW) at the same config, with gradient checkpointing (the reference's shipped setting) and without.  The B200 model
+    clip, torch AdamW) at the same config, with gradient checkpointing (the reference's shipped setting) and without.  The fused model
     must have been freed by the caller.  Baseline being measured — never part of the product path."""
     import torch
     sys.path.insert(0, os.path.join(ROOT, "tools"))
@@ -315,7 +341,7 @@ def library_baseline(dev, cfg, budget_s=150.0):
             out[key] = dict(images_per_s=r["images_per_s"], ms_per_step=r["ms_per_step"], peak_mem_gb=r["peak_mem_gb"])
         except torch.OutOfMemoryError:
             torch.cuda.empty_cache()
-            out[key] = dict(error="out of memory on 180 GB")
+            out[key] = dict(error="out of memory")
     return out
 
 
@@ -383,6 +409,8 @@ def run_b200(args):
     e1.record()
     sync()
     launches = lib.LAUNCHES - n0
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, loss, m, B, host["image_latents"].shape[1])
     my_ms = e0.elapsed_time(e1) / args.steps
     ms = torch.tensor([my_ms], device=dev)
     per_rank = [my_ms]
@@ -394,6 +422,7 @@ def run_b200(args):
     ms_step = ms.item()
     clk = clocks.stop() if rank == 0 else None
     loss_val = float(loss.item())
+    peak_gb = round(torch.cuda.max_memory_allocated(dev) / 2 ** 30, 1)
     # host-side issue time of one step (no synchronisation inside): must stay below the device time, else the GPU starves
     torch.cuda.synchronize()
     th0 = time.perf_counter()
@@ -440,22 +469,15 @@ def run_b200(args):
     del step, opt, m
     torch.cuda.empty_cache()
     kr = kernel_rooflines(dev, B, T, Limg_launch)
-    traffic = None
-    tp = os.path.join(ROOT, "profiles", "r02_ncu_traffic.json")
-    if os.path.exists(tp):
-        traffic = json.load(open(tp))
     g_tf, g_ms, g_fl = kr["gemm"]
     roof = {"bound": "tensor",
-            "kernel": f"gemm2_kernel<256,false,GELU> (CTA pair, cta_group::2): grouped img+txt MLP-up [{B * Limg_launch}+{B * T},3072]x[12288,3072] "
+            "kernel": f"gemm_kernel<256,false,GELU> (wgmma, two consumer warpgroups): grouped img+txt MLP-up [{B * Limg_launch}+{B * T},3072]x[12288,3072] "
                       "with the step's epilogue (GELU output + pre-activation, two [M,4D] bf16 stores)",
             "achieved": g_tf, "peak": burst, "unit": "TFLOP/s", "frac": g_tf / burst, "kernel_ms": g_ms, "flop_per_launch": g_fl,
-            "traffic": (traffic or {}).get("gemm2_mlp_up_gelu", {}).get("dram_bytes") if name == "qwen_edit" else None,  # measured at that shape only
-            "traffic_source": "dram__bytes_read.sum + dram__bytes_write.sum per launch from the ncu --set full capture listed in "
-                              "profiles/r02_ncu_traffic.json" if traffic else None,
-            "peak_source": f"{which} MEASURED_PEAKS.json bf16_tflops (burst; kernels timed alone, L2 flushed between launches)",
+            "peak_source": which,
             "other_kernels": {
-                "attn_bwd (attention_bwd3.cu, pipelined transposed)": {"achieved": kr["attn_bwd"][0], "frac": kr["attn_bwd"][0] / burst, "kernel_ms": kr["attn_bwd"][1]},
-                "attn_fwd (attn_fwd64_kernel)": {"achieved": kr["attn_fwd"][0], "frac": kr["attn_fwd"][0] / burst, "kernel_ms": kr["attn_fwd"][1]}},
+                "attn_bwd (attn_bwd_kernel, transposed scores)": {"achieved": kr["attn_bwd"][0], "frac": kr["attn_bwd"][0] / burst, "kernel_ms": kr["attn_bwd"][1]},
+                "attn_fwd (attn_fwd_kernel)": {"achieved": kr["attn_fwd"][0], "frac": kr["attn_fwd"][0] / burst, "kernel_ms": kr["attn_fwd"][1]}},
             "step_algorithmic_tflops_per_gpu": step_tf, "step_frac_of_sustained": step_tf / sustained, "step_frac_of_burst": step_tf / burst}
     cpu = lib_base = None
     if world == 1 and not args.no_cpu:
@@ -470,9 +492,9 @@ def run_b200(args):
             "data": "synthetic",
             "config": {"workload": cfg["workload"], "name": name, "blocks": n_blocks, "global_batch": B * world, "batch_per_gpu": B,
                        "parallelism": f"dp{world}" + (f"+sharded-frozen-weights({shard_gather}-gather)" if shard else ""),
-                       "l2": "inputs > L2: tens of GB of weights + activations stream through 126 MB L2",
+                       "l2": "inputs > L2: tens of GB of weights + activations stream through the 50 MB L2",
                        "optimizer": "qfx_fused_adamw: global-norm clip 1.0 + AdamW on the LoRA params, one kernel over the flat fp32 gradient",
-                       "loss": loss_val},
+                       "loss": loss_val, "peak_mem_gb": peak_gb},
             "clocks": clk, "gpu_launches": launches, "host_issue_ms_per_step": host_issue_ms, "ms_per_step_per_rank": per_rank, "allreduce": allreduce,
             "e2e": {"value": e2e_ips, "unit": "images/s", "h2d_bytes_per_step": h2d, "d2h_bytes_per_step": 4},
             "roofline": roof, "cpu_baseline": cpu, "library_baseline": lib_base}
@@ -506,6 +528,8 @@ def main():
     ap.add_argument("--layers", type=int, default=0, help="debug only: fewer blocks (INVALID as a bench value)")
     ap.add_argument("--no-cpu", action="store_true", help="skip the cpu_baseline leg")
     ap.add_argument("--no-library", action="store_true", help="skip the library_baseline leg (eager PyTorch on the same GPU)")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write what the last timed step computed (loss, prediction of the target tokens, LoRA gradient and parameters) as .npy files into DIR")
     ap.add_argument("--shard-gather", default="auto", choices=["auto", "peer", "nccl"],
                     help="how a sharded block is assembled: copy-engine pulls from IPC-mapped peer shards (one node) or NCCL all-gather")
     ap.add_argument("--shard-weights", action="store_true",

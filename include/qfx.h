@@ -1,4 +1,4 @@
-/* qfx.h — C ABI of libqfx_b200.so: the B200 (sm_100a) replacement for the reference's per-step hot path
+/* qfx.h — C ABI of libqfx_b200.so: the H100 (sm_90a) replacement for the reference's per-step hot path
  *
  *     noise-predict forward (MMDiT) -> flow-matching MSE -> backward -> LoRA gradients
  *
@@ -24,7 +24,7 @@ const char* qfx_last_error(void);
 int qfx_version(void);
 
 /* ------------------------------------------------------------------------------------------------------------------
- * Fused LoRA projection GEMM (tcgen05 + TMA).  Replaces one `peft.tuners.lora.Linear.forward` call
+ * Fused LoRA projection GEMM (wgmma + TMA).  Replaces one `peft.tuners.lora.Linear.forward` call
  * (injected at base_trainer.py:929-941; y = base(x) + lora_B(lora_A(x)) * alpha/r) or its autograd backward, for
  * up to QFX_MAX_PROBLEMS row-groups that share N, K (e.g. the image and text streams of one MMDiT block:
  * transformer_qwenimage.py:286-293; or the three q|k|v slices of both streams of a LoRA backward, six small problems in one launch).
@@ -33,7 +33,7 @@ int qfx_version(void);
  *   trans_b = 1 :  out[M,N] = epi( alpha * ( A[M,K] . B[K,N]    +  A2[M,64*kb2] . B2[64*kb2,N]   ) )      (dgrad)
  *
  * The LoRA factor pair (A2,B2) is appended to the K loop of the SAME tensor-core contraction (rank padded to a
- * multiple of 64 with zeros by the caller), so one accumulator in TMEM receives base + low-rank update.
+ * multiple of 64 with zeros by the caller), so one register accumulator receives base + low-rank update.
  */
 #define QFX_MAX_PROBLEMS 6
 
@@ -74,7 +74,8 @@ typedef struct {
 } qfx_gemm_problem;
 
 /* lora_group_n > 0 (trans_b = 0 only): output columns [g*lora_group_n, (g+1)*lora_group_n) use A2 columns
- * a2_col0 + g*64*kb2 .. (fused q|k|v projection with one LoRA pair per third).  block_n: 0 = auto, else 64/128/192/256. */
+ * a2_col0 + g*64*kb2 .. (fused q|k|v projection with one LoRA pair per third).  block_n: 0 = auto, else 64/128/192/256
+ * (1000 + 128/256, a request for 256-row CTA-pair tiles, runs as 128/256). */
 int qfx_gemm_bf16(const qfx_gemm_problem* probs, int nprob, int N, int K, int trans_b, int epilogue, float alpha,
                   int lora_group_n, int block_n, void* stream);
 /* out[rows lo..hi) [:, 0:ncols) = 0 for the n_ranges {lo, hi} pairs in `ranges` (device int32): the padding rows a ragged GEMM skips. */
@@ -82,14 +83,14 @@ int qfx_zero_rows(void* out, int64_t ld, int ncols, const int* ranges, int n_ran
 
 
 /* ------------------------------------------------------------------------------------------------------------------
- * Joint text+image attention (head_dim 128), tcgen05.  Q/K/V/dO/dK/dV: [B, H, S, 128] bf16 head-major, text positions
+ * Joint text+image attention (head_dim 128), wgmma.  Q/K/V/dO/dK/dV: [B, H, S, 128] bf16 head-major, text positions
  * first.  Replaces dispatch_attention_fn -> F.scaled_dot_product_attention on the concatenated sequence and its autograd
  * backward (transformer_qwenimage.py:322-345; transformer_flux.py:149-156).  Pad-to-max multi-resolution batches
  * (transformer_qwen_custom.py:444-553, transformer_flux_custom.py:607-616): kv_len (int32 [B], may be NULL) masks keys
  * >= kv_len[b]; txt_len (int32 [B], may be NULL) additionally masks the text padding, keys in [txt_len[b], split).
  * Forward writes O token-major into two row groups: rows with joint position s < split of sample b go to
  * out0[(b*rows0 + s)*ld0 + h*128 ..], the others to out1[(b*rows1 + s - split)*ld1 + h*128 ..]; lse is the log2-domain
- * log-sum-exp [B,H,S].  Backward: dQ_accum is fp32 [B,H,S,128], zeroed by the caller (target of TMA reduce-adds);
+ * log-sum-exp [B,H,S].  Backward: dQ_accum is fp32 [B,H,S,128], zeroed by the caller (every key tile adds into it);
  * delta = rowsum(dO * O) [B,H,S]. */
 int qfx_attn_fwd(const void* Q, const void* K, const void* V, void* out0, int64_t ld0, int rows0, void* out1, int64_t ld1,
                  int rows1, int split, float* lse, const int* kv_len, const int* txt_len, int B, int H, int S,
@@ -178,16 +179,13 @@ int qfx_flow_loss(const void* pred, const void* x0, const void* noise, const flo
 /* G[i*gs_i + j*gs_j] += sum_m P[m,i] Q[m,j], j < r  (LoRA dB = dY^T (sXA^T), dA = (s dY B)^T X); fp32 atomics */
 int qfx_lora_wgrad(const void* P, int64_t ldp, const void* Q, int64_t ldq, float* G, int64_t gs_i, int64_t gs_j, int M, int Dp,
                    int r, void* stream);
-/* The same LoRA weight gradients on the tensor cores (tcgen05, both operands MN-major straight from HBM, rows split over CTAs,
+/* The same LoRA weight gradients on the tensor cores (wgmma, both operands MN-major straight from HBM, rows split over CTAs,
  * fp32 atomics).  A [M, Na] (lda), B [M, 64*G] (ldb), both bf16 row-major; Gp: G device pointers to fp32 gradients.
  *   mode 0: for every group g < G and j < r:  Gp[g][i*gs_i + j*gs_j] += sum_m A[m,i] * B[m, g*64 + j]            (dA, or 1-group dB)
  *   mode 1 (Na = G*Dg): Gp[g][(i - g*Dg)*gs_i + j*gs_j] += sum_m A[m,i] * B[m, g*64 + j]  for g = i / Dg   (dB of a fused q|k|v site)
  * Na % 128 == 0. */
 int qfx_lora_wgrad_tc(const void* A, int64_t lda, int Na, const void* B, int64_t ldb, int G, int M, int mode, int Dg,
                       float* const* Gp, int64_t gs_i, int64_t gs_j, int r, void* stream);
-/* Debugging aid for tools/attn_timeline.py: device buffer of >= 16 * n_query_tiles int64 that receives clock64 stamps of one
- * backward CTA (NULL disables, the default). */
-void qfx_attn_bwd_set_debug(long long* buf);
 /* out = bf16(g * pre_scale * min(1, max_norm / (||g * pre_scale|| + 1e-6)))  (clip_grad_norm_, base_trainer.py:449-455);
  * sumsq receives ||g*pre_scale||^2.  max_norm <= 0 disables clipping. */
 int qfx_grad_finalize(const float* g, int64_t n, float pre_scale, float max_norm, float* sumsq, void* out_bf16, void* stream);

@@ -12,7 +12,7 @@ are not installable here (no network).  tests/shims/ restates ONLY the leaf laye
 FeedForward, Timesteps/TimestepEmbedding, Attention container, SDPA dispatch, rotary helpers, PEFT LoRA Linear, scheduler tables);
 with them, tests/golden/make_ref_model_golden.py runs the REFERENCE'S OWN `qflux.models.transformer_qwenimage`, `transformer_flux`,
 `transformer_qwen_custom`, `transformer_flux_custom`, `BaseTrainer.add_lora_adapter`, `QwenImageEditTrainer._compute_loss` and
-`FluxKontextLoraTrainer._compute_loss` (shared + multi-resolution) and commits their outputs (tests/golden/ref_model_golden.pt).
+`FluxKontextLoraTrainer._compute_loss` (shared + multi-resolution) and commits their outputs (tests/golden/ref_model_golden_*.pt).
 tests/test_reference_goldens.py holds this file to those vectors at fp32 round-off (pred / loss 1e-5, every LoRA gradient 1e-4) on
 ten cases (stock + custom models, Edit-Plus 3-image RoPE, every LoRA target set, all three losses).  What remains un-pinned is the
 dozen leaf ops of tests/shims (no diffusers wheel exists offline to check them against); the loss functions are pinned directly to
@@ -243,7 +243,7 @@ def qwen_rope_per_sample(q, k, rope_list, T, img_offset="aligned"):
     img_offset: where the image table is applied.  "reference" = joint positions [txt_len_b, txt_len_b + L_b) — what the reference does
     (:199-208: `seq_txt` is the per-sample text length, not the padded one), which is mis-aligned by T - txt_len_b whenever a sample's
     text is padded; "aligned" = [T, T + L_b), the positions the image tokens actually occupy.  The two agree when no text is padded
-    (the only case the reference's tests cover, tests/src/models/test_qwen_per_sample_rope.py); the B200 path implements "aligned",
+    (the only case the reference's tests cover, tests/src/models/test_qwen_per_sample_rope.py); the fused path implements "aligned",
     which is what makes a padded batch equal the per-sample un-padded runs."""
     qo, ko = q.clone(), k.clone()
     for b, (img_f, txt_f) in enumerate(rope_list):

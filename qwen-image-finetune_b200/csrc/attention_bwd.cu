@@ -1,402 +1,247 @@
-// Joint attention backward for sm_100a (head_dim 128): dQ, dK, dV from Q, K, V, dO, logsumexp and delta = rowsum(dO*O).
+// Joint attention backward for sm_90a (head_dim 128): dQ, dK, dV from Q, K, V, dO, logsumexp and delta = rowsum(dO*O).
 // This is the autograd backward of F.scaled_dot_product_attention as the reference runs it
 // (/root/reference/src/qflux/models/transformer_qwenimage.py:329-337 under loss.backward(), base_trainer.py:528).
 //
-// One CTA per (128-key tile j, batch*head); it loops over the 128-query tiles i.  All five contractions run on
-// tcgen05 with accumulators in TMEM (512 columns: S|dQ, dP, dV, dK):
-//     S   = Q_i K_j^T          A = Q_i  (K-major)   B = K_j (K-major)
-//     dP  = dO_i V_j^T         A = dO_i (K-major)   B = V_j (K-major)
-//     P   = exp2(S*c - L_i) ;  dS = P o (dP - delta_i) * scale        (compute warps: thread == query row)
-//     dV += P^T  dO_i          A = P   read MN-major (transposed)   B = dO_i read MN-major
-//     dK += dS^T Q_i           A = dS  read MN-major                B = Q_i  read MN-major
-//     dQ_i = dS K_j            A = dS  (K-major)                    B = K_j  read MN-major   -> reuses the S columns
-// The same 128B-swizzled shared-memory tile serves as K-major or MN-major operand — only the descriptor changes — so
-// nothing is transposed in memory.  dQ_i is staged fp32 in the (free) P/dS buffers and added to the global fp32
-// accumulator with one TMA reduce-add (cp.reduce.async.bulk.tensor) per 32-column slab instead of 16K scalar atomics.
+// One CTA per (128-key tile, batch*head), two warpgroups of 64 key rows each; thread 0 also issues the TMA loads (K and V once,
+// a two-stage ring of 64-query tiles of Q and dO).  Scores are TRANSPOSED (row = key), so dK and dV stay in registers:
+//     S^T  = K Q_i^T           wgmma SS   A = K (K-major)                 B = Q_i  (K-major)
+//     dP^T = V dO_i^T          wgmma SS   A = V (K-major)                 B = dO_i (K-major)
+//     P^T  = exp2(S^T c - L_q) ;  dS^T = P^T o (dP^T - delta_q) * scale      (registers; per-query L and delta are per column)
+//     dV  += P^T dO_i          wgmma RS   A = P^T from registers          B = dO_i read MN-major
+//     dK  += dS^T Q_i          wgmma RS   A = dS^T from registers         B = Q_i  read MN-major
+//     dQ_i = dS K              wgmma SS   A = dS^T in shared memory read MN-major, B = K read MN-major; warpgroup w computes
+//                              head-dim columns [64 w, 64 w + 64) over all 128 keys and adds them to the fp32 dQ accumulator with
+//                              8-byte vector reductions (red.global.add.v2.f32) of adjacent column pairs.
+// Keys >= kv_len[b] and text padding [txt_len[b], split) are masked per key ROW; queries past S get L = +inf (P = 0).
 #include <stdlib.h>
 #include <string.h>
 
 #include "../../include/qfx.h"
 #include "host_common.h"
-#include "sm100.cuh"
+#include "sm90.cuh"
 
 namespace qfx {
 
-constexpr int BW_TILE = 128 * 128 * 2;  // 32 KB bf16 tile
-constexpr int BW_ATOM = 128 * 128;      // 16 KB: one 64-wide swizzle atom column of 128 rows
-
 struct AttnBwdParams {
-  CUtensorMap tmQ, tmK, tmV, tmdO;  // bf16 [B*H, S, 128], box {64,128,1}
-  CUtensorMap tmdQ;                 // fp32 [B*H, S, 128], box {32,128,1}  (reduce-add target)
+  CUtensorMap tmK, tmV;    // bf16 [B*H, S, 128], box {64, 128, 1}
+  CUtensorMap tmQ, tmdO;   // bf16 [B*H, S, 128], box {64, 64, 1}
+  float* dQ;               // [B*H, S, 128] fp32, zeroed by the caller: every key tile adds its partial dQ
   bf16* dK;
-  bf16* dV;             // [B*H, S, 128]
-  const float* lse;     // [B*H, S] log2 domain
-  const float* delta;   // [B*H, S]
-  const int* kv_len;    // [B] or NULL: keys >= kv_len[b] masked
-  const int* txt_len;   // [B] or NULL: keys in [txt_len[b], split) masked (text padding)
-  int split;
-  long long* dbg;       // optional: clock64 stamps of CTA (1, 0) — [iteration][16] (tools/attn_timeline.py)
-  int S, H;
+  bf16* dV;
+  const float* lse;        // log2 domain
+  const float* delta;
+  const int* kv_len;
+  const int* txt_len;
+  int split, S, H;
   float scale, scale_log2;
 };
 
-constexpr int BW_SMEM = 7 * BW_TILE + 256;  // K, V, Q x2, dO, P, dS (+ barriers); 1024-aligned base, no slack
+constexpr int BW_KV = 128 * 128 * 2;  // 32 KB: K or V tile, two 64-column swizzle atoms of 16 KB
+constexpr int BW_KV_ATOM = 128 * 128;
+constexpr int BW_Q = 64 * 128 * 2;    // 16 KB: Q_i or dO_i tile, two atoms of 8 KB
+constexpr int BW_Q_ATOM = 64 * 128;
+constexpr int BW_DS = 128 * 64 * 2;   // dS^T [128 keys x 64 queries] bf16, one atom per key row
+constexpr int BW_SMEM = 2 * BW_KV + 4 * BW_Q + BW_DS + 1024 /*align slack*/ + 256;
 
-__device__ __forceinline__ void tma_reduce_add_3d(const CUtensorMap* m, uint32_t src, int c0, int c1, int c2) {
-  asm volatile("cp.reduce.async.bulk.tensor.3d.global.shared::cta.add.bulk_group [%0, {%2, %3, %4}], [%1];" ::"l"(m), "r"(src),
-               "r"(c0), "r"(c1), "r"(c2)
-               : "memory");
+__device__ __forceinline__ uint32_t mul_bf16x2(uint32_t a, uint32_t b) {
+  uint32_t r;
+  asm("mul.rn.bf16x2 %0, %1, %2;" : "=r"(r) : "r"(a), "r"(b));
+  return r;
 }
 
-__device__ __forceinline__ void mask_scores_bwd(uint32_t* r, int col0, int valid, int gap0, int gap1) {
-#pragma unroll
-  for (int i = 0; i < 32; ++i) {
-    const int k = col0 + i;
-    if (!(k < valid) || (k >= gap0 && k < gap1)) r[i] = 0xff800000u;  // -inf
-  }
-}
+__global__ void __launch_bounds__(256, 1) attn_bwd_kernel(const __grid_constant__ AttnBwdParams P) {
+  extern __shared__ uint8_t smem_raw[];
+  const uint32_t smem_base = (smem_u32(smem_raw) + 1023u) & ~1023u;
+  const uint32_t sK = smem_base, sV = smem_base + BW_KV;
+  auto sQ = [&](int st) { return smem_base + 2 * BW_KV + st * BW_Q; };
+  auto sdO = [&](int st) { return smem_base + 2 * BW_KV + (2 + st) * BW_Q; };
+  const uint32_t sdS = smem_base + 2 * BW_KV + 4 * BW_Q;
+  const uint32_t bar_base = sdS + BW_DS;
+  const uint32_t kv_full = bar_base;
+  auto q_full = [&](int st) { return bar_base + 8u * (1 + st); };
 
-// Pipeline per query tile i (key tile fixed per CTA):
-//   MMA     : S = Q_i K^T, dP = dO_i V^T                 -> s_full
-//   compute : P = exp2(S c - L)  -> smem                    -> p_full      (thread = query row x 64 key columns)
-//   MMA     : dV += P^T dO_i                                -> do_empty    (dO_{i+1} starts loading)
-//   compute : dS = P (dP - delta) scale -> smem (over P, after dv_done)  -> ds_full
-//   MMA     : dK += dS^T Q_i  -> q_empty[i&1] ;  dQ_i = dS K (into the S columns)  -> dq_full
-//   compute : dQ_i TMEM -> fp32 slabs parked in the consumed Q_i slot + the dS buffer -> dq_empty (S_{i+1}/dP_{i+1} may issue)
-//             -> TMA reduce-add -> stage_free / qstage_free   (P is not aliased: the next P pass overlaps the reduce)
-// Q is double-buffered and dO is released right after dV, so the loads of tile i+1 hide behind the math of tile i.
-__global__ void __launch_bounds__(320, 1) attn_bwd_kernel(const __grid_constant__ AttnBwdParams P) {
-  extern __shared__ __align__(1024) uint8_t smem_raw[];
-  const uint32_t smem_base = smem_u32(smem_raw);
-  if ((smem_base & 1023u) != 0) __trap();
-  const uint32_t sK = smem_base, sV = smem_base + BW_TILE, sdO = smem_base + 4 * BW_TILE;
-  auto sQ = [&](int st) { return smem_base + (2 + st) * BW_TILE; };
-  const uint32_t sP = smem_base + 5 * BW_TILE, sdS = smem_base + 6 * BW_TILE;
-  const uint32_t bar_base = smem_base + 7 * BW_TILE;
-  const uint32_t kv_full = bar_base, do_full = bar_base + 8, do_empty = bar_base + 16, s_full = bar_base + 24;
-  const uint32_t p_full = bar_base + 32, ds_full = bar_base + 40, dq_full = bar_base + 48, dq_empty = bar_base + 56;
-  const uint32_t stage_free = bar_base + 64, acc_full = bar_base + 72;
-  auto q_full = [&](int st) { return bar_base + 80 + 8u * st; };
-  auto q_empty = [&](int st) { return bar_base + 96 + 8u * st; };
-  auto qstage_free = [&](int st) { return bar_base + 112 + 8u * st; };  // dQ reduce finished reading the slabs parked in Q slot st
-  const uint32_t dq_staged = bar_base + 128;  // all 8 compute warps have parked their dQ slabs in shared memory
-  const uint32_t dv_done = bar_base + 136;    // dV_i has consumed P: the P buffer may be overwritten with dS
-  const uint32_t tmem_slot = bar_base + 144;
-  uint8_t* smem_gen = smem_raw;
-
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int kv0 = blockIdx.x * 128;
   const int bh = blockIdx.y;
   const int b = bh / P.H;
   const int kv_len = P.kv_len ? P.kv_len[b] : P.S;
-  const int n_q = (P.S + 127) / 128;
   const int txt_len = P.txt_len ? P.txt_len[b] : P.split;
-  // a fully masked key tile (beyond kv_len, or entirely inside the text padding) contributes nothing: write zeros and leave
+  // query tiles that hold only padding rows of a pad-to-max batch (positions >= kv_len[b]) carry dO = 0: nothing to add, skip them
+  const int n_q = ((kv_len < P.S ? kv_len : P.S) + 63) / 64;
+  // a fully masked key tile (beyond kv_len, or entirely inside the text padding) contributes nothing: it writes zeros
   const bool active = kv0 < kv_len && !(kv0 >= txt_len && kv0 + 128 <= P.split);
-  const bool dbg_on = P.dbg != nullptr && blockIdx.x == 1 && blockIdx.y == 0;
-#define DBG(i, e) do { if (dbg_on) P.dbg[(i) * 16 + (e)] = clock64(); } while (0)
 
-  if (warp == 1 && lane == 0) {
-    mbar_init(kv_full, 1);
-    mbar_init(do_full, 1);
-    mbar_init(do_empty, 1);
-    mbar_init(s_full, 1);
-    mbar_init(p_full, 8);
-    mbar_init(ds_full, 8);
-    mbar_init(dq_full, 1);
-    mbar_init(dq_empty, 8);
-    mbar_init(stage_free, 1);
-    mbar_init(dq_staged, 8);
-    mbar_init(dv_done, 1);
-    mbar_init(acc_full, 1);
-    for (int st = 0; st < 2; ++st) {
-      mbar_init(q_full(st), 1);
-      mbar_init(q_empty(st), 1);
-      mbar_init(qstage_free(st), 1);
+  const int cw = threadIdx.x >> 7;
+  const int t = threadIdx.x & 127, w = t >> 5, l = t & 31;
+  float dk[64], dv[64];
+#pragma unroll
+  for (int e = 0; e < 64; ++e) dk[e] = dv[e] = 0.f;
+
+  if (active) {
+    if (threadIdx.x == 0) {
+      mbar_init(kv_full, 1);
+      mbar_init(q_full(0), 1);
+      mbar_init(q_full(1), 1);
+      fence_barrier_init();
     }
-    fence_barrier_init();
-  }
-  if (warp == 0) tmem_alloc(tmem_slot, 512);
-  tc_fence_before();
-  __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *reinterpret_cast<volatile uint32_t*>(smem_gen + (tmem_slot - smem_base));
-  const uint32_t tS = tmem_base, tdP = tmem_base + 128, tdV = tmem_base + 256, tdK = tmem_base + 384;
-
-  if (warp == 0) {
-    // ================================================================= TMA producers: lane 0 = K, V, Q tiles; lane 1 = dO tiles
-    if (lane == 0 && active) {
-      mbar_expect_tx(kv_full, 2 * BW_TILE);
+    __syncthreads();
+    auto load_q = [&](int i) {
+      const int st = i & 1;
+      mbar_expect_tx(q_full(st), 2 * BW_Q);
+      tma_load_3d(sQ(st), &P.tmQ, q_full(st), 0, i * 64, bh);
+      tma_load_3d(sQ(st) + BW_Q_ATOM, &P.tmQ, q_full(st), 64, i * 64, bh);
+      tma_load_3d(sdO(st), &P.tmdO, q_full(st), 0, i * 64, bh);
+      tma_load_3d(sdO(st) + BW_Q_ATOM, &P.tmdO, q_full(st), 64, i * 64, bh);
+    };
+    if (threadIdx.x == 0) {
+      mbar_expect_tx(kv_full, 2 * BW_KV);
       tma_load_3d(sK, &P.tmK, kv_full, 0, kv0, bh);
-      tma_load_3d(sK + BW_ATOM, &P.tmK, kv_full, 64, kv0, bh);
+      tma_load_3d(sK + BW_KV_ATOM, &P.tmK, kv_full, 64, kv0, bh);
       tma_load_3d(sV, &P.tmV, kv_full, 0, kv0, bh);
-      tma_load_3d(sV + BW_ATOM, &P.tmV, kv_full, 64, kv0, bh);
-      for (int i = 0; i < n_q; ++i) {
-        const int st = i & 1;
-        if (i >= 2) {
-          mbar_wait(q_empty(st), ((i - 2) >> 1) & 1);      // dK_{i-2} has consumed Q_{i-2}
-          mbar_wait(qstage_free(st), ((i - 2) >> 1) & 1);  // ... and the dQ_{i-2} slabs parked in this slot have been reduced out
-        }
-        mbar_expect_tx(q_full(st), BW_TILE);
-        tma_load_3d(sQ(st), &P.tmQ, q_full(st), 0, i * 128, bh);
-        tma_load_3d(sQ(st) + BW_ATOM, &P.tmQ, q_full(st), 64, i * 128, bh);
-      }
-    } else if (lane == 1 && active) {
-      for (int i = 0; i < n_q; ++i) {
-        if (i >= 1) mbar_wait(do_empty, (i - 1) & 1);
-        mbar_expect_tx(do_full, BW_TILE);
-        tma_load_3d(sdO, &P.tmdO, do_full, 0, i * 128, bh);
-        tma_load_3d(sdO + BW_ATOM, &P.tmdO, do_full, 64, i * 128, bh);
-      }
-    } else if (lane == 2 && active) {
-      // dQ reducer: a thread of its own, so that waiting for the TMA reduce-add to drain shared memory never stalls a compute warp
-      for (int i = 0; i < n_q; ++i) {
-        mbar_wait(dq_staged, i & 1);
-#pragma unroll
-        for (int sl = 0; sl < 4; ++sl)
-          tma_reduce_add_3d(&P.tmdQ, sl < 2 ? sQ(i & 1) + sl * BW_ATOM : sdS + (sl - 2) * BW_ATOM, sl * 32, i * 128, bh);
-        asm volatile("cp.async.bulk.commit_group;" ::: "memory");
-        DBG(i, 14);
-        asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory");
-        mbar_arrive(stage_free);
-        mbar_arrive(qstage_free(i & 1));
-        DBG(i, 15);
-      }
-      asm volatile("cp.async.bulk.wait_group 0;" ::: "memory");  // all reduce-adds have been performed before the CTA exits
+      tma_load_3d(sV + BW_KV_ATOM, &P.tmV, kv_full, 64, kv0, bh);
+      load_q(0);
+      if (n_q > 1) load_q(1);
     }
-  } else if (warp == 1) {
-    // ================================================================= MMA issuer
-    if (lane == 0 && active) {
-      constexpr uint32_t id_kk = idesc_bf16(128, 128, 0, 0);  // A K-major, B K-major
-      constexpr uint32_t id_mm = idesc_bf16(128, 128, 1, 1);  // A MN-major, B MN-major
-      constexpr uint32_t id_km = idesc_bf16(128, 128, 0, 1);  // A K-major, B MN-major
-      auto kmaj = [](uint32_t base, int k) { return sdesc_sw128(base + (k >> 2) * BW_ATOM + (k & 3) * 32, 16, 1024); };
-      auto mnmaj = [](uint32_t base, int k) { return sdesc_sw128(base + k * 2048, BW_ATOM, 1024); };
-      mbar_wait(kv_full, 0);
-      for (int i = 0; i < n_q; ++i) {
-        const int st = i & 1;
-        const uint32_t q = sQ(st);
-        mbar_wait(q_full(st), (i >> 1) & 1);
-        mbar_wait(do_full, i & 1);
-        DBG(i, 0);
-        if (i > 0) mbar_wait(dq_empty, (i - 1) & 1);  // S columns (shared with dQ) drained
-        tc_fence_after();
-        DBG(i, 1);
+    bool key_ok[2];
 #pragma unroll
-        for (int k = 0; k < 8; ++k) umma_bf16(tS, kmaj(q, k), kmaj(sK, k), id_kk, k != 0);
-#pragma unroll
-        for (int k = 0; k < 8; ++k) umma_bf16(tdP, kmaj(sdO, k), kmaj(sV, k), id_kk, k != 0);
-        umma_commit(s_full);
-        mbar_wait(p_full, i & 1);
-        tc_fence_after();
-        DBG(i, 2);
-#pragma unroll
-        for (int k = 0; k < 8; ++k) umma_bf16(tdV, mnmaj(sP, k), mnmaj(sdO, k), id_mm, (i | k) != 0);
-        umma_commit(do_empty);  // dO_i no longer needed
-        umma_commit(dv_done);   // ... and neither is P: dS is written over it (the old dS buffer only stages dQ now)
-        mbar_wait(ds_full, i & 1);
-        tc_fence_after();
-        DBG(i, 3);
-#pragma unroll
-        for (int k = 0; k < 8; ++k) umma_bf16(tdK, mnmaj(sP, k), mnmaj(q, k), id_mm, (i | k) != 0);
-        umma_commit(q_empty(st));  // Q_i no longer needed
-#pragma unroll
-        for (int k = 0; k < 8; ++k) umma_bf16(tS, kmaj(sP, k), mnmaj(sK, k), id_km, k != 0);
-        umma_commit(dq_full);
-      }
-      umma_commit(acc_full);
+    for (int hh = 0; hh < 2; ++hh) {
+      const int key = kv0 + cw * 64 + 16 * w + (l >> 2) + 8 * hh;
+      key_ok[hh] = key < kv_len && !(key >= txt_len && key < P.split);
     }
-  } else {
-    // ================================================================= compute warps: 2 per TMEM lane quadrant,
-    // thread = query row x 64 of the 128 key columns (and 64 of the 128 head-dim columns when draining dQ / dK / dV)
-    const int quad = warp & 3;
-    const int half = (warp - 2) >> 2;
-    const int c0 = half * 64;
-    const int row = quad * 32 + lane;
-    const uint32_t lane_off = (uint32_t)(quad * 32) << 16;
-    const int tid = threadIdx.x - 64;  // 0..255
-    if (active) {
-      const int valid = kv_len - kv0;  // key columns >= valid are masked
-      const int gap0 = txt_len - kv0, gap1 = P.split - kv0;  // tile-local text-padding columns [gap0, gap1)
-      const bool full_tile = valid >= 128 && (gap0 >= gap1 || gap0 >= 128 || gap1 <= 0);
-      const uint32_t off_row = (uint32_t)row * 128 + half * BW_ATOM;  // this thread's 64 columns = one swizzle-atom row
-      for (int i = 0; i < n_q; ++i) {
-        const int q = i * 128 + row;
-        const bool q_ok = q < P.S;
-        const float L = q_ok ? P.lse[(int64_t)bh * P.S + q] : INFINITY;
-        const float dls = (q_ok ? P.delta[(int64_t)bh * P.S + q] : 0.f) * P.scale;
-        if (tid == 0) DBG(i, 8);
-        mbar_wait(s_full, i & 1);
-        tc_fence_after();
-        if (tid == 0) DBG(i, 9);
-        float p[64];
-        // ---- pass 1: P
+    const uint32_t aK = sK + cw * 64 * 128, aV = sV + cw * 64 * 128;
+    mbar_wait(kv_full, 0);
+    for (int i = 0; i < n_q; ++i) {
+      const int st = i & 1;
+      const int q0 = i * 64;
+      float sc[32], dp[32];
+      mbar_wait(q_full(st), (i >> 1) & 1);
+      reg_fence(sc, 32);
+      reg_fence(dp, 32);
+      wgmma_fence();
 #pragma unroll
-        for (int cc = 0; cc < 2; ++cc) {
-          uint32_t rs[32];
-          tmem_ld32(tS + lane_off + c0 + cc * 32, rs);
-          tmem_ld_wait();
-          uint32_t pk[16];
-          if (!full_tile) mask_scores_bwd(rs, c0 + cc * 32, valid, gap0, gap1);  // rare: masked keys -> -inf -> P = 0
+      for (int k = 0; k < 8; ++k)
+        wgmma_ss_n64<0, 0>(sc, sdesc_sw128(aK + (k >> 2) * BW_KV_ATOM + (k & 3) * 32, 16, 1024),
+                           sdesc_sw128(sQ(st) + (k >> 2) * BW_Q_ATOM + (k & 3) * 32, 16, 1024), k != 0);
 #pragma unroll
-          for (int e = 0; e < 32; ++e) p[cc * 32 + e] = exp2f(__uint_as_float(rs[e]) * P.scale_log2 - L);
+      for (int k = 0; k < 8; ++k)
+        wgmma_ss_n64<0, 0>(dp, sdesc_sw128(aV + (k >> 2) * BW_KV_ATOM + (k & 3) * 32, 16, 1024),
+                           sdesc_sw128(sdO(st) + (k >> 2) * BW_Q_ATOM + (k & 3) * 32, 16, 1024), k != 0);
+      wgmma_commit();
+      wgmma_wait<0>();
+      reg_fence(sc, 32);
+      reg_fence(dp, 32);
+      // P^T and dS^T, packed as bf16 pairs in the accumulator layout (= the A fragments of the next contractions)
+      uint32_t pa[16], da[16];
 #pragma unroll
-          for (int e = 0; e < 16; ++e) pk[e] = pack_bf16(p[cc * 32 + 2 * e], p[cc * 32 + 2 * e + 1]);
-#pragma unroll
-          for (int v = 0; v < 4; ++v) {
-            const uint32_t chunk = (uint32_t)(cc * 4 + v) ^ (uint32_t)(row & 7);
-            asm volatile("st.shared.v4.b32 [%0], {%1, %2, %3, %4};" ::"r"(sP + off_row + chunk * 16), "r"(pk[4 * v]),
-                         "r"(pk[4 * v + 1]), "r"(pk[4 * v + 2]), "r"(pk[4 * v + 3])
-                         : "memory");
-          }
+      for (int jj = 0; jj < 8; ++jj) {
+        const int q = q0 + 8 * jj + 2 * (l & 3);
+        float2 L = make_float2(INFINITY, INFINITY), D = make_float2(0.f, 0.f);
+        if (q < P.S) {
+          L.x = P.lse[(int64_t)bh * P.S + q];
+          D.x = P.delta[(int64_t)bh * P.S + q];
         }
-        fence_proxy_async_smem();
-        __syncwarp();
-        if (lane == 0) mbar_arrive(p_full);
-        if (tid == 0) DBG(i, 11);
-        // ---- pass 2: dS = P * (dP * scale - delta * scale), written over P once dV_i has consumed it
-        if (tid == 0) DBG(i, 10);
-#pragma unroll
-        for (int cc = 0; cc < 2; ++cc) {
-          uint32_t rp[32];
-          tmem_ld32(tdP + lane_off + c0 + cc * 32, rp);
-          tmem_ld_wait();
-          uint32_t dk[16];
-#pragma unroll
-          for (int e = 0; e < 16; ++e)
-            dk[e] = pack_bf16(p[cc * 32 + 2 * e] * (__uint_as_float(rp[2 * e]) * P.scale - dls),
-                              p[cc * 32 + 2 * e + 1] * (__uint_as_float(rp[2 * e + 1]) * P.scale - dls));
-          if (cc == 0) mbar_wait(dv_done, i & 1);
-#pragma unroll
-          for (int v = 0; v < 4; ++v) {
-            const uint32_t chunk = (uint32_t)(cc * 4 + v) ^ (uint32_t)(row & 7);
-            asm volatile("st.shared.v4.b32 [%0], {%1, %2, %3, %4};" ::"r"(sP + off_row + chunk * 16), "r"(dk[4 * v]),
-                         "r"(dk[4 * v + 1]), "r"(dk[4 * v + 2]), "r"(dk[4 * v + 3])
-                         : "memory");
-          }
+        if (q + 1 < P.S) {
+          L.y = P.lse[(int64_t)bh * P.S + q + 1];
+          D.y = P.delta[(int64_t)bh * P.S + q + 1];
         }
-        fence_proxy_async_smem();
-        tc_fence_before();
-        __syncwarp();
-        if (lane == 0) mbar_arrive(ds_full);
-        if (tid == 0) DBG(i, 12);
-
-        // ---- drain dQ_i: TMEM -> fp32 swizzled slabs in the (now idle) P|dS buffers -> TMA reduce-add to global
-        mbar_wait(dq_full, i & 1);
-        tc_fence_after();
-        if (tid == 0) DBG(i, 13);
-        if (i > 0) mbar_wait(stage_free, (i - 1) & 1);  // the staging buffer of dQ_{i-1} has been reduced out (long ago)
 #pragma unroll
-        for (int cc = 0; cc < 2; ++cc) {
-          uint32_t r[32];
-          const int c = c0 + cc * 32;
-          tmem_ld32(tS + lane_off + c, r);
-          tmem_ld_wait();
-          // [128 rows x 32 fp32] slabs, 128 B rows: head-dim columns 0..63 are parked in the (consumed) Q_i slot, 64..127 in a staging
-          // buffer of their own — nothing the next tile writes is aliased, so its P / dS passes never wait for this reduce
-          const uint32_t slab = (c < 64 ? sQ(i & 1) + (c >> 5) * BW_ATOM : sdS + ((c - 64) >> 5) * BW_ATOM) + (uint32_t)row * 128;
-#pragma unroll
-          for (int v = 0; v < 8; ++v) {
-            const uint32_t chunk = (uint32_t)v ^ (uint32_t)(row & 7);
-            asm volatile("st.shared.v4.b32 [%0], {%1, %2, %3, %4};" ::"r"(slab + chunk * 16), "r"(r[4 * v]), "r"(r[4 * v + 1]),
-                         "r"(r[4 * v + 2]), "r"(r[4 * v + 3])
-                         : "memory");
-          }
-        }
-        tc_fence_before();
-        __syncwarp();
-        if (lane == 0) mbar_arrive(dq_empty);  // the S columns are free: S_{i+1} / dP_{i+1} may issue while the reduce drains
-        if (tid == 0) DBG(i, 7);
-        fence_proxy_async_smem();
-        __syncwarp();
-        if (lane == 0) mbar_arrive(dq_staged);  // the reducer thread (warp 0, lane 2) takes it from here
-      }
-      mbar_wait(acc_full, 0);
-      tc_fence_after();
-    }
-    // ----------------------------------------------------------------- epilogue: dK, dV tiles
-    const int kv = kv0 + row;
-    if (kv0 < P.S) {
-#pragma unroll 1
-      for (int which = 0; which < 2; ++which) {
-        bf16* dst = (which ? P.dK : P.dV) + ((int64_t)bh * P.S + kv) * 128;
-        const uint32_t t = (which ? tdK : tdV) + lane_off;
-#pragma unroll 1
-        for (int c = c0; c < c0 + 64; c += 32) {
-          uint32_t r[32];
-          if (active) {
-            tmem_ld32(t + c, r);
-            tmem_ld_wait();
-          } else {
-#pragma unroll
-            for (int e = 0; e < 32; ++e) r[e] = 0;
-          }
-          if (kv < P.S) {
-            uint4* d4 = reinterpret_cast<uint4*>(dst + c);
-#pragma unroll
-            for (int v = 0; v < 4; ++v)
-              d4[v] = make_uint4(pack_bf16(__uint_as_float(r[8 * v]), __uint_as_float(r[8 * v + 1])),
-                                 pack_bf16(__uint_as_float(r[8 * v + 2]), __uint_as_float(r[8 * v + 3])),
-                                 pack_bf16(__uint_as_float(r[8 * v + 4]), __uint_as_float(r[8 * v + 5])),
-                                 pack_bf16(__uint_as_float(r[8 * v + 6]), __uint_as_float(r[8 * v + 7])));
-          }
+        for (int hh = 0; hh < 2; ++hh) {
+          const int r = 4 * jj + 2 * hh;
+          uint32_t p = pack_bf16(exp2f(sc[r] * P.scale_log2 - L.x), exp2f(sc[r + 1] * P.scale_log2 - L.y));
+          if (!key_ok[hh]) p = 0u;
+          // dS = P o (dP c - delta c): the bracket in fp32, rounded to bf16 and multiplied by the bf16 P as a packed pair
+          const uint32_t d = mul_bf16x2(p, pack_bf16(dp[r] * P.scale - D.x * P.scale, dp[r + 1] * P.scale - D.y * P.scale));
+          pa[2 * jj + hh] = p;
+          da[2 * jj + hh] = d;
         }
       }
+      // dS^T to shared memory: [128 keys][64 queries], 128B-swizzled rows (the MN-major A operand of dQ)
+#pragma unroll
+      for (int jj = 0; jj < 8; ++jj)
+#pragma unroll
+        for (int hh = 0; hh < 2; ++hh) {
+          const int kr = cw * 64 + 16 * w + (l >> 2) + 8 * hh;
+          const uint32_t addr = sdS + kr * 128 + ((uint32_t)(jj ^ (kr & 7)) << 4) + (l & 3) * 4;
+          asm volatile("st.shared.b32 [%0], %1;" ::"r"(addr), "r"(da[2 * jj + hh]) : "memory");
+        }
+      fence_proxy_async_smem();
+      // A fragment of k-chunk c (queries 16 c ..): {pair(jj = 2c, h 0), pair(2c, h 1), pair(2c + 1, h 0), pair(2c + 1, h 1)}
+      reg_fence(dv, 64);
+      reg_fence(dk, 64);
+      wgmma_fence();
+#pragma unroll
+      for (int c = 0; c < 4; ++c) wgmma_rs_n128<1>(dv, pa + 4 * c, sdesc_sw128(sdO(st) + c * 2048, BW_Q_ATOM, 1024), 1);
+#pragma unroll
+      for (int c = 0; c < 4; ++c) wgmma_rs_n128<1>(dk, da + 4 * c, sdesc_sw128(sQ(st) + c * 2048, BW_Q_ATOM, 1024), 1);
+      wgmma_commit();
+      named_bar(1, 256);  // dS^T of both warpgroups is in shared memory
+      float dq[32];
+      reg_fence(dq, 32);
+      wgmma_fence();
+#pragma unroll
+      for (int c = 0; c < 8; ++c)
+        wgmma_ss_n64<1, 1>(dq, sdesc_sw128(sdS + c * 2048, BW_Q_ATOM, 1024), sdesc_sw128(sK + cw * BW_KV_ATOM + c * 2048, BW_KV_ATOM, 1024),
+                           c != 0);
+      wgmma_commit();
+      wgmma_wait<0>();
+      reg_fence(dq, 32);
+      reg_fence(dv, 64);
+      reg_fence(dk, 64);
+#pragma unroll
+      for (int hh = 0; hh < 2; ++hh) {
+        const int q = q0 + 16 * w + (l >> 2) + 8 * hh;
+        if (q < P.S) {
+          float* dst = P.dQ + ((int64_t)bh * P.S + q) * 128 + cw * 64 + 2 * (l & 3);
+#pragma unroll
+          for (int jj = 0; jj < 8; ++jj) red_add_v2(dst + 8 * jj, dq[4 * jj + 2 * hh], dq[4 * jj + 2 * hh + 1]);
+        }
+      }
+      named_bar(1, 256);  // stage st and the dS^T buffer are free
+      if (threadIdx.x == 0 && i + 2 < n_q) load_q(i + 2);
     }
   }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 0) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, 512);
+  // epilogue: dK, dV rows of this warpgroup's 64 keys (zeros for a fully masked key tile)
+#pragma unroll
+  for (int hh = 0; hh < 2; ++hh) {
+    const int key = kv0 + cw * 64 + 16 * w + (l >> 2) + 8 * hh;
+    if (key >= P.S) continue;
+    bf16* dK = P.dK + ((int64_t)bh * P.S + key) * 128 + 2 * (l & 3);
+    bf16* dV = P.dV + ((int64_t)bh * P.S + key) * 128 + 2 * (l & 3);
+#pragma unroll
+    for (int jj = 0; jj < 16; ++jj) {
+      *reinterpret_cast<uint32_t*>(dK + 8 * jj) = pack_bf16(dk[4 * jj + 2 * hh], dk[4 * jj + 2 * hh + 1]);
+      *reinterpret_cast<uint32_t*>(dV + 8 * jj) = pack_bf16(dv[4 * jj + 2 * hh], dv[4 * jj + 2 * hh + 1]);
+    }
   }
 }
 
-int make_qkv_tmap(CUtensorMap* m, const void* base, int BH, int S);
+int make_qkv_tmap(CUtensorMap* m, const void* base, int BH, int S);  // attention_fwd.cu
+
+static int make_q64_tmap(CUtensorMap* m, const void* base, int BH, int S) {
+  uint64_t dims[3] = {128, (uint64_t)S, (uint64_t)BH};
+  uint64_t strides[2] = {128 * 2, (uint64_t)S * 128 * 2};
+  uint32_t box[3] = {64, 64, 1};
+  return make_tmap_bf16(m, base, 3, dims, strides, box);
+}
 
 }  // namespace qfx
 
 using namespace qfx;
 
-long long* g_qfx_attn_bwd_dbg = nullptr;
-/* debugging aid: device buffer of >= 16 * n_query_tiles int64 that receives clock64 stamps of CTA (1,0) (NULL disables) */
-extern "C" void qfx_attn_bwd_set_debug(long long* buf) { g_qfx_attn_bwd_dbg = buf; }
-
-/* All of Q, K, V, dO, dK, dV: [B, H, S, 128] bf16; dQ_accum: [B, H, S, 128] fp32, MUST be zeroed by the caller (it is the
- * target of TMA reduce-adds from every key tile).  lse: log2-domain logsumexp from qfx_attn_fwd; delta = rowsum(dO*O). */
-namespace qfx {
-int attn_bwd_pipelined(const void* Q, const void* K, const void* V, const void* dO, const float* lse, const float* delta, float* dQ,
-                       void* dK, void* dV, const int* kv_len, const int* txt_len, int split, int B, int H, int S, float softmax_scale,
-                       cudaStream_t stream);  // attention_bwd3.cu
-}
-
+/* All of Q, K, V, dO, dK, dV: [B, H, S, 128] bf16; dQ_accum: [B, H, S, 128] fp32, MUST be zeroed by the caller (every key tile
+ * adds its partial dQ into it).  lse: log2-domain logsumexp from qfx_attn_fwd; delta = rowsum(dO*O). */
 extern "C" int qfx_attn_bwd(const void* Q, const void* K, const void* V, const void* dO, const float* lse, const float* delta,
                             float* dQ_accum, void* dK, void* dV, const int* kv_len, const int* txt_len, int split, int B, int H,
                             int S, float softmax_scale, void* stream) {
-  extern long long* g_qfx_attn_bwd_dbg;
   QFX_CHECK_ARG(B > 0 && H > 0 && S > 0 && dQ_accum && dK && dV && lse && delta, "qfx_attn_bwd: bad arguments");
-  // default: the software-pipelined transposed kernel (attention_bwd3.cu).  A/B switch: QFX_ATTN_BWD1=1 runs the round-1 serial-chain
-  // kernel below (the same-box comparison in profiles/r02_bench_b_*.json).  The 64-query transposed variant of round 1 lives on as
-  // tools/experiments/attention_bwd_transposed_64q.cu — it never beat either and is no longer part of the library.
-  static const bool serial = getenv("QFX_ATTN_BWD1") != nullptr;
-  if (!serial)
-    return qfx::attn_bwd_pipelined(Q, K, V, dO, lse, delta, dQ_accum, dK, dV, kv_len, txt_len, split, B, H, S, softmax_scale,
-                                   (cudaStream_t)stream);
   AttnBwdParams P;
   memset(&P, 0, sizeof(P));
   int rc;
-  if ((rc = make_qkv_tmap(&P.tmQ, Q, B * H, S))) return rc;
   if ((rc = make_qkv_tmap(&P.tmK, K, B * H, S))) return rc;
   if ((rc = make_qkv_tmap(&P.tmV, V, B * H, S))) return rc;
-  if ((rc = make_qkv_tmap(&P.tmdO, dO, B * H, S))) return rc;
-  {
-    uint64_t dims[3] = {128, (uint64_t)S, (uint64_t)(B * H)};
-    uint64_t strides[2] = {128 * 4, (uint64_t)S * 128 * 4};
-    uint32_t box[3] = {32, 128, 1};
-    if ((rc = make_tmap_f32(&P.tmdQ, dQ_accum, 3, dims, strides, box))) return rc;
-  }
-  P.dK = (bf16*)dK; P.dV = (bf16*)dV; P.lse = lse; P.delta = delta; P.kv_len = kv_len; P.txt_len = txt_len; P.split = txt_len ? split : 0; P.S = S; P.H = H;
-  P.dbg = g_qfx_attn_bwd_dbg;
+  if ((rc = make_q64_tmap(&P.tmQ, Q, B * H, S))) return rc;
+  if ((rc = make_q64_tmap(&P.tmdO, dO, B * H, S))) return rc;
+  P.dQ = dQ_accum; P.dK = (bf16*)dK; P.dV = (bf16*)dV; P.lse = lse; P.delta = delta; P.kv_len = kv_len; P.txt_len = txt_len;
+  P.split = txt_len ? split : 0; P.S = S; P.H = H;
   P.scale = softmax_scale;
   P.scale_log2 = softmax_scale * 1.4426950408889634f;
   static bool attr_done = false;
@@ -405,7 +250,7 @@ extern "C" int qfx_attn_bwd(const void* Q, const void* K, const void* V, const v
     attr_done = true;
   }
   dim3 grid((S + 127) / 128, B * H);
-  attn_bwd_kernel<<<grid, 320, BW_SMEM, (cudaStream_t)stream>>>(P);
+  attn_bwd_kernel<<<grid, 256, BW_SMEM, (cudaStream_t)stream>>>(P);
   QFX_CUDA(cudaGetLastError());
   return 0;
 }

@@ -1,22 +1,18 @@
-// Joint (text+image) non-causal attention forward for sm_100a, head_dim 128, bf16 in / fp32 softmax.
+// Joint (text+image) non-causal attention forward for sm_90a, head_dim 128, bf16 in / fp32 softmax.
 // Replaces `dispatch_attention_fn` -> F.scaled_dot_product_attention on the concatenated [txt; img] sequence
 // (/root/reference/src/qflux/models/transformer_qwenimage.py:322-345, transformer_flux.py:149-156).
 //
-// One CTA per (128-query tile, batch*head).  Roles: warp 0 = TMEM alloc + TMA producer, warp 1 = MMA issuer,
-// warps 2-9 = softmax: two warps per TMEM lane quadrant, each thread owns one query row x 64 of the 128 key columns
-// (row max / row sum are combined across the pair through shared memory).  Per 128-key tile j:
-//     S[j%2] = Q K_j^T            tcgen05.mma SS, both operands K-major (d contiguous), accumulator in TMEM
-//     P      = exp2(S*c - m)      softmax warps: tcgen05.ld, row max / sum in registers, bf16 P -> swizzled smem
-//     O     += P V_j              tcgen05.mma SS, A = P (K-major), B = V (MN-major: d contiguous), accumulate in TMEM
-// QK^T of tile j+1 is issued before P V of tile j so the tensor pipe works while the softmax warps run.
-// O is rescaled in TMEM only when the running max grows by more than 2^8 (warp-uniform decision), as the final
-// normalisation by the running sum makes a stale max exact.
+// One CTA per (128-query tile, batch*head), two warpgroups of 64 query rows each; thread 0 also issues the TMA loads of a
+// two-stage K / V ring.  Per 128-key tile j:
+//     S   = Q K_j^T          wgmma SS, both operands K-major (d contiguous), fp32 accumulator in registers
+//     P   = exp2(S*c - m)    in registers; row max / sum reduced over the four threads of a quad
+//     O  += P V_j            wgmma RS: A = P straight from the accumulator registers (bf16), B = V (MN-major: d contiguous)
 #include <stdlib.h>
 #include <string.h>
 
 #include "../../include/qfx.h"
 #include "host_common.h"
-#include "sm100.cuh"
+#include "sm90.cuh"
 
 namespace qfx {
 
@@ -28,7 +24,6 @@ constexpr int ATOM_BYTES = 128 * 128;      // 16 KB
 
 struct AttnFwdParams {
   CUtensorMap tmQ, tmK, tmV;  // [B*H, S, 128] bf16, box {64, 128, 1}
-  CUtensorMap tmK64, tmV64;   // same tensors, box {64, 64, 1} (64-key tiles of the two-CTAs-per-SM kernel)
   bf16* out0;                 // rows with joint position s < split  -> out0[(b*rows0 + s) * ld0 + h*128 ..]
   bf16* out1;                 // rows with s >= split               -> out1[(b*rows1 + s - split) * ld1 + h*128 ..]
   int64_t ld0, ld1;
@@ -40,17 +35,7 @@ struct AttnFwdParams {
   float scale_log2;    // (1/sqrt(d)) * log2(e)
 };
 
-constexpr int ATT_SMEM = 7 * TILE_BYTES + 256 + 2 * 2 * 128 * 4;  // Q, K x2, V x2, P x2, barriers, row-max exchange
-
-// Key masking happens OUTSIDE the hot loops: in the (rare) partially valid tile the masked scores are overwritten with -inf, so
-// the max / exp2 loops carry no predicates (the if-converted per-element compares doubled the softmax instruction count).
-__device__ __forceinline__ void mask_scores(uint32_t* r, int col0, int valid, int gap0, int gap1) {
-#pragma unroll
-  for (int i = 0; i < 32; ++i) {
-    const int k = col0 + i;
-    if (!(k < valid) || (k >= gap0 && k < gap1)) r[i] = 0xff800000u;  // -inf
-  }
-}
+constexpr int ATT_SMEM = 5 * TILE_BYTES + 1024 /*align slack*/ + 256;  // Q, K x2, V x2, barriers
 
 // A query tile that holds only padding rows of a pad-to-max batch (every query position >= kv_len[b], all of them image rows): the
 // output rows become zeros (they feed row-wise kernels and must stay finite) and no attention math runs.
@@ -67,469 +52,134 @@ __device__ __forceinline__ bool attn_fwd_skip_padding_tile(const AttnFwdParams& 
   return true;
 }
 
-__global__ void __launch_bounds__(320, 1) attn_fwd_kernel(const __grid_constant__ AttnFwdParams P) {
-  extern __shared__ __align__(1024) uint8_t smem_raw[];  // 128B-swizzle atoms need 1024 B alignment (no slack left to round up)
-  const uint32_t smem_base = smem_u32(smem_raw);
-  if ((smem_base & 1023u) != 0) __trap();
+__global__ void __launch_bounds__(256, 1) attn_fwd_kernel(const __grid_constant__ AttnFwdParams P) {
+  extern __shared__ uint8_t smem_raw[];
+  const uint32_t smem_base = (smem_u32(smem_raw) + 1023u) & ~1023u;  // 128B-swizzle atoms need 1024 B alignment
   const uint32_t sQ = smem_base;
   auto sK = [&](int s) { return smem_base + TILE_BYTES * (1 + s); };
   auto sV = [&](int s) { return smem_base + TILE_BYTES * (3 + s); };
-  auto sP = [&](int s) { return smem_base + TILE_BYTES * (5 + s); };
-  const uint32_t bar_base = smem_base + 7 * TILE_BYTES;
+  const uint32_t bar_base = smem_base + 5 * TILE_BYTES;
   const uint32_t q_full = bar_base;
-  auto k_full = [&](int s) { return bar_base + 8u * (1 + s); };
-  auto v_full = [&](int s) { return bar_base + 8u * (3 + s); };
-  auto s_full = [&](int s) { return bar_base + 8u * (5 + s); };
-  auto p_full = [&](int s) { return bar_base + 8u * (7 + s); };
-  auto pv_done = [&](int s) { return bar_base + 8u * (9 + s); };
-  const uint32_t o_full = bar_base + 8u * 11;
-  auto k_empty = [&](int s) { return bar_base + 8u * (12 + s); };
-  const uint32_t tmem_slot = bar_base + 8u * 14;
-  const uint32_t red_base = bar_base + 256;  // float red[2 (tile parity)][2 (half)][128 rows]
-  uint8_t* smem_gen = smem_raw + (smem_base - smem_u32(smem_raw));
+  auto kv_full = [&](int s) { return bar_base + 8u * (1 + s); };
 
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int q0 = blockIdx.x * ATT_BQ;
-  const int bh = blockIdx.y;
-  const int b = bh / P.H, h = bh - b * P.H;
-  const int kv_len = P.kv_len ? P.kv_len[b] : P.S;
-  const int txt_len = P.txt_len ? P.txt_len[b] : P.split;  // >= 1; keys [txt_len, split) are text padding
-  const int n_tiles = (kv_len + ATT_BK - 1) / ATT_BK;
-  if (attn_fwd_skip_padding_tile(P, q0, b, h, bh, kv_len)) return;
-
-  if (warp == 1 && lane == 0) {
-    mbar_init(q_full, 1);
-    for (int s = 0; s < 2; ++s) {
-      mbar_init(k_full(s), 1);
-      mbar_init(v_full(s), 1);
-      mbar_init(s_full(s), 1);
-      mbar_init(p_full(s), 8);
-      mbar_init(pv_done(s), 1);
-      mbar_init(k_empty(s), 1);
-    }
-    mbar_init(o_full, 1);
-    fence_barrier_init();
-  }
-  if (warp == 0) tmem_alloc(tmem_slot, 512);
-  tc_fence_before();
-  __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *reinterpret_cast<volatile uint32_t*>(smem_gen + (tmem_slot - smem_base));
-  const uint32_t tS0 = tmem_base, tO = tmem_base + 256;
-
-  if (warp == 0) {
-    // ================================================================= TMA producers: lane 0 streams Q + K tiles, lane 1 streams V
-    // tiles (independent threads so a wait on a V stage never delays the next K load)
-    if (lane == 0) {
-      tma_prefetch_desc(&P.tmQ);
-      tma_prefetch_desc(&P.tmK);
-      mbar_expect_tx(q_full, TILE_BYTES);
-      tma_load_3d(sQ, &P.tmQ, q_full, 0, q0, bh);
-      tma_load_3d(sQ + ATOM_BYTES, &P.tmQ, q_full, 64, q0, bh);
-      for (int j = 0; j < n_tiles; ++j) {
-        const int s = j & 1;
-        // K stage s is free as soon as Q K^T of tile j-2 has completed (long before its P V): the K load of tile j then overlaps
-        // the softmax of tile j-2, so the next Q K^T never waits on HBM/L2 latency
-        if (j >= 2) mbar_wait(k_empty(s), ((j - 2) >> 1) & 1);
-        mbar_expect_tx(k_full(s), TILE_BYTES);
-        tma_load_3d(sK(s), &P.tmK, k_full(s), 0, j * ATT_BK, bh);
-        tma_load_3d(sK(s) + ATOM_BYTES, &P.tmK, k_full(s), 64, j * ATT_BK, bh);
-      }
-    } else if (lane == 1) {
-      tma_prefetch_desc(&P.tmV);
-      for (int j = 0; j < n_tiles; ++j) {
-        const int s = j & 1;
-        if (j >= 2) mbar_wait(pv_done(s), ((j - 2) >> 1) & 1);  // P V of tile j-2 finished reading V stage s
-        mbar_expect_tx(v_full(s), TILE_BYTES);
-        tma_load_3d(sV(s), &P.tmV, v_full(s), 0, j * ATT_BK, bh);
-        tma_load_3d(sV(s) + ATOM_BYTES, &P.tmV, v_full(s), 64, j * ATT_BK, bh);
-      }
-    }
-  } else if (warp == 1) {
-    // ================================================================= MMA issuer
-    if (lane == 0) {
-      constexpr uint32_t idesc_qk = idesc_bf16(128, 128, 0, 0);
-      constexpr uint32_t idesc_pv = idesc_bf16(128, 128, 0, 1);
-      mbar_wait(q_full, 0);
-      auto issue_pv = [&](int j) {
-        const int s = j & 1;
-        mbar_wait(p_full(s), (j >> 1) & 1);
-        mbar_wait(v_full(s), (j >> 1) & 1);
-        tc_fence_after();
-#pragma unroll
-        for (int k = 0; k < 8; ++k) {
-          const uint64_t ad = sdesc_sw128(sP(s) + (k >> 2) * ATOM_BYTES + (k & 3) * 32, 16, 1024);
-          const uint64_t bd = sdesc_sw128(sV(s) + k * 2048, ATOM_BYTES, 1024);
-          umma_bf16(tO, ad, bd, idesc_pv, (j | k) != 0);
-        }
-        umma_commit(pv_done(s));
-      };
-      for (int j = 0; j < n_tiles; ++j) {
-        const int s = j & 1;
-        mbar_wait(k_full(s), (j >> 1) & 1);
-        tc_fence_after();
-        // S[s] is free: p_full(s) of tile j-2 (== softmax finished reading S[s]) was waited before P V (j-2) was issued
-#pragma unroll
-        for (int k = 0; k < 8; ++k) {
-          const uint64_t ad = sdesc_sw128(sQ + (k >> 2) * ATOM_BYTES + (k & 3) * 32, 16, 1024);
-          const uint64_t bd = sdesc_sw128(sK(s) + (k >> 2) * ATOM_BYTES + (k & 3) * 32, 16, 1024);
-          umma_bf16(tS0 + s * 128, ad, bd, idesc_qk, k != 0);
-        }
-        umma_commit(s_full(s));
-        umma_commit(k_empty(s));
-        if (j > 0) issue_pv(j - 1);
-      }
-      issue_pv(n_tiles - 1);
-      umma_commit(o_full);
-    }
-  } else {
-    // ================================================================= softmax warps (thread = query row x 64 key columns)
-    const int quad = warp & 3;
-    const int half = (warp - 2) >> 2;  // 0: columns 0..63, 1: columns 64..127 of every tile (and of O in the epilogue)
-    const int row = quad * 32 + lane;
-    const uint32_t lane_off = (uint32_t)(quad * 32) << 16;
-    const int c0 = half * 64;
-    float* red = reinterpret_cast<float*>(smem_gen + (red_base - smem_base));
-    auto pair_sync = [&]() { asm volatile("bar.sync %0, 64;" ::"r"(1 + quad) : "memory"); };
-    float m_used = -INFINITY, l = 0.f;
-    for (int j = 0; j < n_tiles; ++j) {
-      const int s = j & 1;
-      const int valid = kv_len - j * ATT_BK;  // columns >= valid are masked
-      const int gap0 = txt_len - j * ATT_BK, gap1 = P.split - j * ATT_BK;  // tile-local text-padding range [gap0, gap1)
-      mbar_wait(s_full(s), (j >> 1) & 1);
-      tc_fence_after();
-      const uint32_t tS = tS0 + s * 128 + lane_off + c0;
-      float mx = -INFINITY;
-      // warp-uniform: no key masking needed (all tiles but the last, unless the tile touches text padding)
-      const bool full_tile = valid >= ATT_BK && (gap0 >= gap1 || gap0 >= ATT_BK || gap1 <= 0);
-#pragma unroll 1
-      for (int c = 0; c < 64; c += 32) {
-        uint32_t r[32];
-        tmem_ld32(tS + c, r);
-        tmem_ld_wait();
-        if (!full_tile) mask_scores(r, c0 + c, valid, gap0, gap1);  // rare (last tile / text padding): masked keys -> -inf
-#pragma unroll
-        for (int i = 0; i < 32; ++i) mx = fmaxf(mx, __uint_as_float(r[i]));
-      }
-      red[(s * 2 + half) * 128 + row] = mx;
-      pair_sync();
-      mx = fmaxf(mx, red[(s * 2 + (half ^ 1)) * 128 + row]);
-      // (a tile that is entirely text padding leaves mx = -inf: m_new = m_used, all p = 0 — tile 0 always has a valid key)
-      const float m_new = fmaxf(m_used, mx * P.scale_log2);
-      // warp-uniform lazy rescale of the TMEM accumulator (both warps of a pair see the same rows -> same decision)
-      const bool need = (j == 0) || (m_new > m_used + 8.f);
-      if (__any_sync(0xffffffffu, need)) {
-        if (j > 0) {
-          mbar_wait(pv_done((j - 1) & 1), ((j - 1) >> 1) & 1);  // all earlier P V MMAs have landed in O
-          tc_fence_after();
-          const float alpha = exp2f(m_used - m_new);
-#pragma unroll 1
-          for (int c = 0; c < 64; c += 32) {
-            uint32_t r[32];
-            tmem_ld32(tO + lane_off + c0 + c, r);
-            tmem_ld_wait();
-#pragma unroll
-            for (int i = 0; i < 32; ++i) r[i] = __float_as_uint(__uint_as_float(r[i]) * alpha);
-            tmem_st32(tO + lane_off + c0 + c, r);
-          }
-          tmem_st_wait();
-          l *= alpha;
-        }
-        m_used = m_new;
-      }
-      if (j >= 2) mbar_wait(pv_done(s), ((j - 2) >> 1) & 1);  // P buffer s no longer read by the tensor core
-      const uint32_t p_row = sP(s) + half * ATOM_BYTES + row * 128;  // this thread's 64 columns = one swizzle atom row
-      float lsum = 0.f;
-#pragma unroll 1
-      for (int c = 0; c < 64; c += 32) {
-        uint32_t r[32];
-        tmem_ld32(tS + c, r);
-        tmem_ld_wait();
-        uint32_t pk[16];
-        if (!full_tile) mask_scores(r, c0 + c, valid, gap0, gap1);  // exp2(-inf) = 0 for masked keys
-#pragma unroll
-        for (int i = 0; i < 16; ++i) {
-          const float p0 = exp2f(__uint_as_float(r[2 * i]) * P.scale_log2 - m_used);
-          const float p1 = exp2f(__uint_as_float(r[2 * i + 1]) * P.scale_log2 - m_used);
-          pk[i] = pack_bf16(p0, p1);
-          lsum += p0 + p1;
-        }
-#pragma unroll
-        for (int v = 0; v < 4; ++v) {
-          const uint32_t chunk = (uint32_t)((c >> 3) + v) ^ (uint32_t)(row & 7);
-          asm volatile("st.shared.v4.b32 [%0], {%1, %2, %3, %4};" ::"r"(p_row + chunk * 16), "r"(pk[4 * v]), "r"(pk[4 * v + 1]),
-                       "r"(pk[4 * v + 2]), "r"(pk[4 * v + 3])
-                       : "memory");
-        }
-      }
-      l += lsum;
-      fence_proxy_async_smem();
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(p_full(s));
-    }
-    // ----------------------------------------------------------------- epilogue: O / l -> bf16, token-major
-    pair_sync();  // everyone is done with the row-max slots: reuse slot 0 for the partial row sums
-    red[half * 128 + row] = l;
-    pair_sync();
-    l += red[(half ^ 1) * 128 + row];
-    mbar_wait(o_full, 0);
-    tc_fence_after();
-    const int sq = q0 + row;
-    const bool ok = sq < P.S;
-    const float inv = 1.f / l;
-    bf16* dst = nullptr;
-    if (ok) {
-      dst = (sq < P.split ? P.out0 + ((int64_t)b * P.rows0 + sq) * P.ld0 + h * ATT_D
-                          : P.out1 + ((int64_t)b * P.rows1 + (sq - P.split)) * P.ld1 + h * ATT_D) + c0;
-      if (P.lse && half == 0) P.lse[(int64_t)bh * P.S + sq] = m_used + log2f(l);
-    }
-#pragma unroll 1
-    for (int c = 0; c < 64; c += 32) {
-      uint32_t r[32];
-      tmem_ld32(tO + lane_off + c0 + c, r);
-      tmem_ld_wait();
-      if (ok) {
-        uint4* d4 = reinterpret_cast<uint4*>(dst + c);
-#pragma unroll
-        for (int v = 0; v < 4; ++v)
-          d4[v] = make_uint4(pack_bf16(__uint_as_float(r[8 * v]) * inv, __uint_as_float(r[8 * v + 1]) * inv),
-                             pack_bf16(__uint_as_float(r[8 * v + 2]) * inv, __uint_as_float(r[8 * v + 3]) * inv),
-                             pack_bf16(__uint_as_float(r[8 * v + 4]) * inv, __uint_as_float(r[8 * v + 5]) * inv),
-                             pack_bf16(__uint_as_float(r[8 * v + 6]) * inv, __uint_as_float(r[8 * v + 7]) * inv));
-      }
-    }
-  }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 0) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, 512);
-  }
-}
-
-// =====================================================================================================================
-// 64-key-tile variant, TWO CTAs resident per SM.  The 128-key kernel above is latency bound: every tile walks the chain
-// S ready -> tcgen05.ld -> max -> exp2 (MUFU) -> st.shared -> fence -> P V, and its 224 KB of shared memory leave the SM to a
-// single CTA.  Here a CTA needs 112 KB of shared memory and 256 TMEM columns (S 2 x 64, O 128), so two CTAs share an SM and the
-// tensor pipe of one runs under the softmax of the other.  4 softmax warps, thread = query row x all 64 keys of the tile (one TMEM
-// round trip per tile, no cross-warp exchange).  K is released right after Q K^T, V after P V.  P never touches shared memory:
-// the softmax thread packs its row to bf16 and stores it with tcgen05.st over the first 32 columns of the S buffer it was read
-// from, and P V runs with the A operand in tensor memory.  (The kernel is shared-memory-bandwidth bound — SS-mode operands at
-// 128 B/clk/SM — and P through shared memory cost a 16 KB store plus a 16 KB operand read per 64-key tile.)
-constexpr int F64_KT = 64 * 128 * 2;                                 // one K or V tile: 64 keys x 128 dims = 16 KB (two 8 KB atoms)
-constexpr int F64_SMEM = TILE_BYTES + 4 * F64_KT + 256;  // Q + K x2 + V x2 + barriers = 96.25 KB
-
-__global__ void __launch_bounds__(192, 2) attn_fwd64_kernel(const __grid_constant__ AttnFwdParams P) {
-  extern __shared__ __align__(1024) uint8_t smem_raw[];
-  const uint32_t smem_base = smem_u32(smem_raw);
-  if ((smem_base & 1023u) != 0) __trap();
-  const uint32_t sQ = smem_base;
-  auto sK = [&](int s) { return smem_base + TILE_BYTES + F64_KT * s; };
-  auto sV = [&](int s) { return smem_base + TILE_BYTES + F64_KT * (2 + s); };
-  const uint32_t bar_base = smem_base + TILE_BYTES + 4 * F64_KT;
-  const uint32_t q_full = bar_base;
-  auto k_full = [&](int s) { return bar_base + 8u * (1 + s); };
-  auto v_full = [&](int s) { return bar_base + 8u * (3 + s); };
-  auto s_full = [&](int s) { return bar_base + 8u * (5 + s); };
-  // ONE barrier per S/P buffer: S(j+1) is issued before P V(j), so with a single barrier a fast softmax warp could arrive for tile j+1
-  // before a slow one has arrived for tile j, completing tile j's phase without it — the P V(j) MMA then read fp32 score bits as bf16 P
-  // (round-2 finding: a latent race of the round-1 kernel, exposed as sporadic NaNs once the MMA issue got faster)
-  auto p_full = [&](int s) { return bar_base + 8u * (14 + s); };
-  auto pv_done = [&](int s) { return bar_base + 8u * (8 + s); };
-  const uint32_t o_full = bar_base + 8u * 10;
-  auto k_empty = [&](int s) { return bar_base + 8u * (11 + s); };
-  const uint32_t tmem_slot = bar_base + 8u * 13;
-  uint8_t* smem_gen = smem_raw;
-
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int q0 = blockIdx.x * ATT_BQ;
   const int bh = blockIdx.y;
   const int b = bh / P.H, h = bh - b * P.H;
   const int kv_len = P.kv_len ? P.kv_len[b] : P.S;
   const int txt_len = P.txt_len ? P.txt_len[b] : P.split;
-  const int n_tiles = (kv_len + 63) / 64;
+  const int n_tiles = (kv_len + ATT_BK - 1) / ATT_BK;
   if (attn_fwd_skip_padding_tile(P, q0, b, h, bh, kv_len)) return;
 
-  if (warp == 1 && lane == 0) {
+  if (threadIdx.x == 0) {
     mbar_init(q_full, 1);
-    for (int s = 0; s < 2; ++s) {
-      mbar_init(k_full(s), 1);
-      mbar_init(v_full(s), 1);
-      mbar_init(s_full(s), 1);
-      mbar_init(pv_done(s), 1);
-      mbar_init(k_empty(s), 1);
-    }
-    mbar_init(p_full(0), 4);
-    mbar_init(p_full(1), 4);
-    mbar_init(o_full, 1);
+    mbar_init(kv_full(0), 1);
+    mbar_init(kv_full(1), 1);
     fence_barrier_init();
   }
-  if (warp == 0) tmem_alloc(tmem_slot, 256);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *reinterpret_cast<volatile uint32_t*>(smem_gen + (tmem_slot - smem_base));
-  const uint32_t tS0 = tmem_base, tO = tmem_base + 128;
-
-  if (warp == 0) {
-    // ================================================================= TMA producers: lane 0 = Q + K tiles, lane 1 = V tiles
-    if (lane == 0) {
-      tma_prefetch_desc(&P.tmQ);
-      tma_prefetch_desc(&P.tmK64);
-      mbar_expect_tx(q_full, TILE_BYTES);
-      tma_load_3d(sQ, &P.tmQ, q_full, 0, q0, bh);
-      tma_load_3d(sQ + ATOM_BYTES, &P.tmQ, q_full, 64, q0, bh);
-      for (int j = 0; j < n_tiles; ++j) {
-        const int s = j & 1;
-        if (j >= 2) mbar_wait(k_empty(s), ((j - 2) >> 1) & 1);
-        mbar_expect_tx(k_full(s), F64_KT);
-        tma_load_3d(sK(s), &P.tmK64, k_full(s), 0, j * 64, bh);
-        tma_load_3d(sK(s) + 8192, &P.tmK64, k_full(s), 64, j * 64, bh);
-      }
-    } else if (lane == 1) {
-      tma_prefetch_desc(&P.tmV64);
-      for (int j = 0; j < n_tiles; ++j) {
-        const int s = j & 1;
-        if (j >= 2) mbar_wait(pv_done(s), ((j - 2) >> 1) & 1);
-        mbar_expect_tx(v_full(s), F64_KT);
-        tma_load_3d(sV(s), &P.tmV64, v_full(s), 0, j * 64, bh);
-        tma_load_3d(sV(s) + 8192, &P.tmV64, v_full(s), 64, j * 64, bh);
-      }
-    }
-  } else if (warp == 1) {
-    // ================================================================= MMA issuer: the whole warp runs the loop with identical values and an
-    // elected lane issues (sm100.cuh umma_ss_w / umma_ts_w): a 64-key S instruction is only 32 clk of tensor work, and the single-lane issue
-    // region of round 1 spent ~19 SASS instructions (lane-serialising loop, R2UR per operand) on each
-    {
-      constexpr uint32_t idesc_qk = idesc_bf16(128, 64, 0, 0);
-      constexpr uint32_t idesc_pv = idesc_bf16(128, 128, 0, 1);
-      const uint32_t kQ = sdesc_lo(sQ, 16);
-      mbar_wait(q_full, 0);
-      auto issue_pv = [&](int j) {
-        const int s = j & 1;
-        const uint32_t mV = sdesc_lo(sV(s), 8192);
-        mbar_wait(p_full(s), (j >> 1) & 1);
-        mbar_wait(v_full(s), (j >> 1) & 1);
-        tc_fence_after();
-#pragma unroll
-        for (int k = 0; k < 4; ++k)  // K = 64 keys: P in TMEM (8 packed columns per 16 keys), V MN-major (two 64-wide d atoms, 8 KB apart)
-          umma_ts_w(tO, tS0 + s * 64 + k * 8, mV + (uint32_t)(k * 128), idesc_pv, (j | k) != 0);
-        umma_commit_w(pv_done(s));
-      };
-      for (int j = 0; j < n_tiles; ++j) {
-        const int s = j & 1;
-        const uint32_t kK = sdesc_lo(sK(s), 16);
-        mbar_wait(k_full(s), (j >> 1) & 1);
-        tc_fence_after();
-#pragma unroll
-        for (int k = 0; k < 8; ++k)
-          umma_ss_w(tS0 + s * 64, kQ + (uint32_t)((k >> 2) * 1024 + (k & 3) * 2), kK + (uint32_t)((k >> 2) * 512 + (k & 3) * 2), idesc_qk, k != 0);
-        umma_commit_w(s_full(s));
-        umma_commit_w(k_empty(s));
-        if (j > 0) issue_pv(j - 1);
-      }
-      issue_pv(n_tiles - 1);
-      umma_commit_w(o_full);
-    }
-  } else {
-    // ================================================================= softmax warps (thread = query row)
-    const int quad = warp & 3;
-    const int row = quad * 32 + lane;
-    const uint32_t lane_off = (uint32_t)(quad * 32) << 16;
-    float m_used = -INFINITY, l = 0.f;
-    for (int j = 0; j < n_tiles; ++j) {
-      const int s = j & 1;
-      const int valid = kv_len - j * 64;
-      const int gap0 = txt_len - j * 64, gap1 = P.split - j * 64;
-      const bool full_tile = valid >= 64 && (gap0 >= gap1 || gap0 >= 64 || gap1 <= 0);
-      mbar_wait(s_full(s), (j >> 1) & 1);
-      tc_fence_after();
-      uint32_t r[64];
-      tmem_ld32(tS0 + s * 64 + lane_off, r);
-      tmem_ld32(tS0 + s * 64 + lane_off + 32, r + 32);
-      tmem_ld_wait();
-      if (!full_tile) {
-        mask_scores(r, 0, valid, gap0, gap1);
-        mask_scores(r + 32, 32, valid, gap0, gap1);
-      }
-      // four independent chains: with two softmax warps per scheduler a 64-deep dependent FMNMX / FADD chain is pure latency
-      float mx4[4] = {-INFINITY, -INFINITY, -INFINITY, -INFINITY};
-#pragma unroll
-      for (int i = 0; i < 64; ++i) mx4[i & 3] = fmaxf(mx4[i & 3], __uint_as_float(r[i]));
-      const float mx = fmaxf(fmaxf(mx4[0], mx4[1]), fmaxf(mx4[2], mx4[3]));
-      const float m_new = fmaxf(m_used, mx * P.scale_log2);  // a fully padded tile: mx = -inf, m_new = m_used (tile 0 has a valid key)
-      if (__any_sync(0xffffffffu, (j == 0) || (m_new > m_used + 8.f))) {  // warp-uniform lazy rescale
-        if (j > 0) {
-          mbar_wait(pv_done((j - 1) & 1), ((j - 1) >> 1) & 1);
-          tc_fence_after();
-          const float alpha = exp2f(m_used - m_new);
-#pragma unroll 1
-          for (int c = 0; c < 128; c += 32) {
-            uint32_t o[32];
-            tmem_ld32(tO + lane_off + c, o);
-            tmem_ld_wait();
-#pragma unroll
-            for (int i = 0; i < 32; ++i) o[i] = __float_as_uint(__uint_as_float(o[i]) * alpha);
-            tmem_st32(tO + lane_off + c, o);
-          }
-          tmem_st_wait();
-          l *= alpha;
-        }
-        m_used = m_new;
-      }
-      uint32_t pk[32];
-      float ls4[4] = {0.f, 0.f, 0.f, 0.f};
-#pragma unroll
-      for (int i = 0; i < 32; ++i) {
-        // (all exponentials on MUFU: routing 1/8 .. 1/2 of them through exp2_fma was measured 3-15 % slower — sm100.cuh)
-        const float p0 = exp2f(__uint_as_float(r[2 * i]) * P.scale_log2 - m_used);
-        const float p1 = exp2f(__uint_as_float(r[2 * i + 1]) * P.scale_log2 - m_used);
-        pk[i] = pack_bf16(p0, p1);
-        ls4[i & 3] += p0 + p1;
-      }
-      l += (ls4[0] + ls4[1]) + (ls4[2] + ls4[3]);
-      // P_j over the S_j columns this thread has already read (its own TMEM lane).  The buffer is not rewritten before S_{j+2},
-      // which the MMA thread issues after P V_j.
-      tmem_st32(tS0 + s * 64 + lane_off, pk);
-      tmem_st_wait();
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(p_full(s));
-    }
-    // ----------------------------------------------------------------- epilogue
-    mbar_wait(o_full, 0);
-    tc_fence_after();
-    const int sq = q0 + row;
-    const bool ok = sq < P.S;
-    const float inv = 1.f / l;
-    bf16* dst = nullptr;
-    if (ok) {
-      dst = sq < P.split ? P.out0 + ((int64_t)b * P.rows0 + sq) * P.ld0 + h * ATT_D
-                         : P.out1 + ((int64_t)b * P.rows1 + (sq - P.split)) * P.ld1 + h * ATT_D;
-      if (P.lse) P.lse[(int64_t)bh * P.S + sq] = m_used + log2f(l);
-    }
-#pragma unroll 1
-    for (int c = 0; c < 128; c += 32) {
-      uint32_t o[32];
-      tmem_ld32(tO + lane_off + c, o);
-      tmem_ld_wait();
-      if (ok) {
-        uint4* d4 = reinterpret_cast<uint4*>(dst + c);
-#pragma unroll
-        for (int v = 0; v < 4; ++v)
-          d4[v] = make_uint4(pack_bf16(__uint_as_float(o[8 * v]) * inv, __uint_as_float(o[8 * v + 1]) * inv),
-                             pack_bf16(__uint_as_float(o[8 * v + 2]) * inv, __uint_as_float(o[8 * v + 3]) * inv),
-                             pack_bf16(__uint_as_float(o[8 * v + 4]) * inv, __uint_as_float(o[8 * v + 5]) * inv),
-                             pack_bf16(__uint_as_float(o[8 * v + 6]) * inv, __uint_as_float(o[8 * v + 7]) * inv));
-      }
-    }
+  auto load_kv = [&](int j) {
+    const int s = j & 1;
+    mbar_expect_tx(kv_full(s), 2 * TILE_BYTES);
+    tma_load_3d(sK(s), &P.tmK, kv_full(s), 0, j * ATT_BK, bh);
+    tma_load_3d(sK(s) + ATOM_BYTES, &P.tmK, kv_full(s), 64, j * ATT_BK, bh);
+    tma_load_3d(sV(s), &P.tmV, kv_full(s), 0, j * ATT_BK, bh);
+    tma_load_3d(sV(s) + ATOM_BYTES, &P.tmV, kv_full(s), 64, j * ATT_BK, bh);
+  };
+  if (threadIdx.x == 0) {
+    tma_prefetch_desc(&P.tmQ);
+    tma_prefetch_desc(&P.tmK);
+    tma_prefetch_desc(&P.tmV);
+    mbar_expect_tx(q_full, TILE_BYTES);
+    tma_load_3d(sQ, &P.tmQ, q_full, 0, q0, bh);
+    tma_load_3d(sQ + ATOM_BYTES, &P.tmQ, q_full, 64, q0, bh);
+    load_kv(0);
+    if (n_tiles > 1) load_kv(1);
   }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 0) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, 256);
+
+  const int cw = threadIdx.x >> 7;  // warpgroup: query rows 64 cw .. + 63 of the tile
+  const int t = threadIdx.x & 127, w = t >> 5, l = t & 31;
+  float o[64], sc[64];
+#pragma unroll
+  for (int e = 0; e < 64; ++e) o[e] = 0.f;
+  float m_used[2] = {-INFINITY, -INFINITY}, lsum[2] = {0.f, 0.f};
+  mbar_wait(q_full, 0);
+  const uint32_t aQ = sQ + cw * 64 * 128;
+  for (int j = 0; j < n_tiles; ++j) {
+    const int s = j & 1;
+    mbar_wait(kv_full(s), (j >> 1) & 1);
+    reg_fence(sc, 64);
+    wgmma_fence();
+#pragma unroll
+    for (int k = 0; k < 8; ++k)
+      wgmma_ss_n128<0, 0>(sc, sdesc_sw128(aQ + (k >> 2) * ATOM_BYTES + (k & 3) * 32, 16, 1024),
+                          sdesc_sw128(sK(s) + (k >> 2) * ATOM_BYTES + (k & 3) * 32, 16, 1024), k != 0);
+    wgmma_commit();
+    wgmma_wait<0>();
+    reg_fence(sc, 64);
+    // keys >= kv_len[b] and the text padding [txt_len[b], split) are masked (only tiles that contain such keys pay for the test)
+    const int k0 = j * ATT_BK;
+    if (k0 + ATT_BK > kv_len || (txt_len < P.split && k0 < P.split && k0 + ATT_BK > txt_len)) {
+#pragma unroll
+      for (int jj = 0; jj < 16; ++jj)
+#pragma unroll
+        for (int e = 0; e < 2; ++e) {
+          const int key = k0 + 8 * jj + 2 * (l & 3) + e;
+          if (key >= kv_len || (key >= txt_len && key < P.split)) sc[4 * jj + e] = sc[4 * jj + 2 + e] = -INFINITY;
+        }
+    }
+#pragma unroll
+    for (int hh = 0; hh < 2; ++hh) {
+      float mx = -INFINITY;
+#pragma unroll
+      for (int jj = 0; jj < 16; ++jj) mx = fmaxf(mx, fmaxf(sc[4 * jj + 2 * hh], sc[4 * jj + 2 * hh + 1]));
+      mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 1));
+      mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 2));
+      const float m_new = fmaxf(m_used[hh], mx * P.scale_log2);
+      const float m_safe = m_new == -INFINITY ? 0.f : m_new;  // a row with no valid key so far: all its p are 0
+      const float alpha = exp2f(m_used[hh] - m_safe);
+      m_used[hh] = m_new;
+      lsum[hh] *= alpha;
+#pragma unroll
+      for (int jj = 0; jj < 16; ++jj) {
+        o[4 * jj + 2 * hh] *= alpha;
+        o[4 * jj + 2 * hh + 1] *= alpha;
+        const float p0 = exp2f(sc[4 * jj + 2 * hh] * P.scale_log2 - m_safe);
+        const float p1 = exp2f(sc[4 * jj + 2 * hh + 1] * P.scale_log2 - m_safe);
+        sc[4 * jj + 2 * hh] = p0;
+        sc[4 * jj + 2 * hh + 1] = p1;
+        lsum[hh] += p0 + p1;
+      }
+    }
+    uint32_t pa[32];
+#pragma unroll
+    for (int c = 0; c < 8; ++c)
+#pragma unroll
+      for (int e = 0; e < 4; ++e) pa[4 * c + e] = pack_bf16(sc[8 * c + 2 * e], sc[8 * c + 2 * e + 1]);
+    reg_fence(o, 64);
+    wgmma_fence();
+#pragma unroll
+    for (int c = 0; c < 8; ++c) wgmma_rs_n128<1>(o, pa + 4 * c, sdesc_sw128(sV(s) + c * 2048, ATOM_BYTES, 1024), 1);
+    wgmma_commit();
+    wgmma_wait<0>();
+    reg_fence(o, 64);
+    named_bar(1, 256);  // both warpgroups are done with stage s
+    if (threadIdx.x == 0 && j + 2 < n_tiles) load_kv(j + 2);
+  }
+  // ----------------------------------------------------------------- epilogue
+#pragma unroll
+  for (int hh = 0; hh < 2; ++hh) {
+    float ls = lsum[hh];
+    ls += __shfl_xor_sync(0xffffffffu, ls, 1);
+    ls += __shfl_xor_sync(0xffffffffu, ls, 2);
+    const int sq = q0 + cw * 64 + 16 * w + (l >> 2) + 8 * hh;
+    if (sq >= P.S) continue;
+    const float inv = 1.f / ls;
+    bf16* dst = sq < P.split ? P.out0 + ((int64_t)b * P.rows0 + sq) * P.ld0 + h * ATT_D
+                             : P.out1 + ((int64_t)b * P.rows1 + (sq - P.split)) * P.ld1 + h * ATT_D;
+    if (P.lse && (l & 3) == 0) P.lse[(int64_t)bh * P.S + sq] = m_used[hh] + log2f(ls);
+#pragma unroll
+    for (int jj = 0; jj < 16; ++jj)
+      *reinterpret_cast<uint32_t*>(dst + 8 * jj + 2 * (l & 3)) = pack_bf16(o[4 * jj + 2 * hh] * inv, o[4 * jj + 2 * hh + 1] * inv);
   }
 }
 
@@ -550,8 +200,6 @@ extern "C" int qfx_attn_fwd(const void* Q, const void* K, const void* V, void* o
                             int64_t ld1, int rows1, int split, float* lse, const int* kv_len, const int* txt_len, int B, int H,
                             int S, float softmax_scale, void* stream) {
   QFX_CHECK_ARG(B > 0 && H > 0 && S > 0 && out0 && (split >= S || out1), "qfx_attn_fwd: bad arguments");
-  // default: the 64-key-tile kernel (two CTAs per SM).  A/B switch: QFX_ATTN_FWD128=1 the first 128-key-tile kernel.  The two-query-tiles-
-  // per-CTA ping-pong design (341 us vs 266) is kept for the record as tools/experiments/attention_fwd_two_tiles.cu, outside the library.
   AttnFwdParams P;
   memset(&P, 0, sizeof(P));
   int rc;
@@ -562,29 +210,13 @@ extern "C" int qfx_attn_fwd(const void* Q, const void* K, const void* V, void* o
   P.ld0 = ld0; P.ld1 = ld1; P.rows0 = rows0; P.rows1 = rows1; P.split = split;
   P.lse = lse; P.kv_len = kv_len; P.txt_len = txt_len; P.S = S; P.H = H;
   P.scale_log2 = softmax_scale * 1.4426950408889634f;
-  static const bool use128 = getenv("QFX_ATTN_FWD128") != nullptr;  // A/B switch: the single-CTA-per-SM 128-key-tile kernel
-  dim3 grid((S + ATT_BQ - 1) / ATT_BQ, B * H);
-  if (!use128) {
-    uint64_t dims[3] = {128, (uint64_t)S, (uint64_t)(B * H)};
-    uint64_t strides[2] = {128 * 2, (uint64_t)S * 128 * 2};
-    uint32_t box[3] = {64, 64, 1};
-    if ((rc = make_tmap_bf16(&P.tmK64, K, 3, dims, strides, box))) return rc;
-    if ((rc = make_tmap_bf16(&P.tmV64, V, 3, dims, strides, box))) return rc;
-    static bool attr64 = false;
-    if (!attr64) {
-      QFX_CUDA(cudaFuncSetAttribute(attn_fwd64_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, F64_SMEM));
-      attr64 = true;
-    }
-    attn_fwd64_kernel<<<grid, 192, F64_SMEM, (cudaStream_t)stream>>>(P);
-    QFX_CUDA(cudaGetLastError());
-    return 0;
-  }
   static bool attr_done = false;
   if (!attr_done) {
     QFX_CUDA(cudaFuncSetAttribute(attn_fwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, ATT_SMEM));
     attr_done = true;
   }
-  attn_fwd_kernel<<<grid, 320, ATT_SMEM, (cudaStream_t)stream>>>(P);
+  dim3 grid((S + ATT_BQ - 1) / ATT_BQ, B * H);
+  attn_fwd_kernel<<<grid, 256, ATT_SMEM, (cudaStream_t)stream>>>(P);
   QFX_CUDA(cudaGetLastError());
   return 0;
 }

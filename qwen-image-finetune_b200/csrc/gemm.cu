@@ -1,5 +1,5 @@
-// Fused LoRA projection GEMM for sm_100a: persistent, warp-specialised, TMA -> 128B-swizzled smem ring ->
-// tcgen05.mma (M=128 x N=BN x K=16, fp32 accumulators double-buffered in TMEM) -> epilogue warps (tcgen05.ld).
+// Fused LoRA projection GEMM for sm_90a: persistent, warp-specialised, TMA -> 128B-swizzled smem ring ->
+// wgmma (two consumer warpgroups, each M=64 x N=BN x K=16 with fp32 accumulators in registers) -> fused epilogue.
 //
 // Replaces the reference's `peft` LoRA Linear forward / backward-dgrad on the MMDiT block projections
 // (/root/reference/src/qflux/models/transformer_qwenimage.py:286-293,348-352 and FeedForward :408,418; LoRA injected
@@ -7,11 +7,11 @@
 // same contraction as extra 64-wide k-blocks taken from a second pair of tensor maps, so each projection is ONE
 // tensor-core contraction:   acc = X.W^T + (s X A^T).B^T   (forward)   |   acc = dY.W + (s dY B).A   (dgrad).
 //
-// Roles (256 threads, 1 CTA / SM): warp 0 = TMA producer, warp 1 = MMA issuer, warp 2 = TMEM allocator,
-// warps 4-7 = epilogue (warp w owns TMEM lanes 32*(w%4) .. +31 = output rows).
+// Roles (384 threads, 1 CTA / SM): warpgroup 0 = TMA producer (one thread), warpgroups 1-2 = consumers: rows 64*(wg-1) .. +63
+// of the 128-row tile.  The producer runs ahead into the next tile's k-blocks while the consumers run the epilogue.
 #include "../../include/qfx.h"
 #include "host_common.h"
-#include "sm100.cuh"
+#include "sm90.cuh"
 #include <stdlib.h>
 #include <string.h>
 
@@ -42,15 +42,8 @@ struct GemmParams {  // passed by value as a __grid_constant__ kernel parameter:
   int tiles_m_end[QFX_MAX_PROBLEMS];  // running sum of the problems' m-tile counts (problem i owns m-tiles [end[i-1], end[i]))
   int tiles_m_total, tiles_n, total_tiles;
   float alpha;
-  // split-K of the last, partial wave of the CTA-pair kernel (tail_split > 1): tiles >= tail_first are cut into tail_split
-  // K ranges that run on otherwise idle CTA pairs; partial sums meet in tail_ws (fp32, zeroed by a memset node in front of the
-  // launch) and the CTA whose arrival completes tail_cnt runs the epilogue of its half tile
-  int tail_first, tail_split;
-  int n_fast;  // CTA-pair kernel: consecutive tiles walk N first (A rows stay in L2) instead of M first (B tile stays)
   int stream_out;  // epilogue stores bypass L2 residency (st.global.cs): set when the output is larger than L2, so that writing it does not
                    // evict the A operand every wave re-reads (ncu, round 1: 658 MB of DRAM reads for 210 MB of operands on the MLP-up GEMM)
-  float* tail_ws;
-  int* tail_cnt;
 };
 
 static_assert(sizeof(GemmParams) <= 4090, "GemmParams must fit the kernel parameter space");
@@ -61,8 +54,10 @@ struct GemmCfg {
   static constexpr int B_BYTES = BN * BK * 2;
   static constexpr int STAGE_BYTES = A_BYTES + B_BYTES;
   static constexpr int STAGES = BN == 256 ? 4 : BN == 192 ? 5 : BN == 128 ? 6 : 8;
-  static constexpr int TMEM_COLS = 2 * BN <= 128 ? 128 : 2 * BN <= 256 ? 256 : 512;
-  static constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + 1024 /*align slack*/ + 256 /*barriers*/;
+  static constexpr int EPI_LD = 33;  // fp32 staging row of one 32-column chunk, padded: row-per-thread reads are conflict-free
+  static constexpr int EPI_BYTES = 2 * 64 * EPI_LD * 4;
+  static constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + EPI_BYTES + 1024 /*align slack*/ + 256 /*barriers*/;
+  static_assert(SMEM_BYTES <= 227 * 1024, "shared memory of one CTA");
 };
 
 __device__ __forceinline__ void st_out(uint4* p, uint4 v, bool stream) {
@@ -70,204 +65,167 @@ __device__ __forceinline__ void st_out(uint4* p, uint4 v, bool stream) {
   else *p = v;
 }
 
-// Epilogue of one [128 x BN] accumulator tile: thread = output row (TMEM lane), 32 columns per tcgen05.ld.
-// ws_row != nullptr: the accumulator row comes from the split-K workspace (fp32, global) instead of tensor memory
-template <int BN, int EPI>
-__device__ __forceinline__ void epilogue_tile(const GemmProb& q, const GemmParams& P, uint32_t t_row, int row, bool row_ok, int n0,
-                                              float* ws_row = nullptr) {
-    const bf16* gate_row = nullptr;
-    if (EPI == QFX_EPI_RESID_GATE && row_ok) gate_row = q.gate + (int64_t)(row / q.rows_per_batch) * q.ldg;
-    // ATTN_DO: this row is token (ab, as) of the joint sequence; dacc carries sum_d dO*O across the four 32-column chunks of a head
-    int ab = 0, as = 0;
-    float dacc = 0.f;
-    if (EPI == QFX_EPI_ATTN_DO) {
-      ab = row / q.rows_per_batch;
-      as = q.s_offset + row - ab * q.rows_per_batch;
-    }
-#pragma unroll 1
-    for (int c = 0; c < BN; c += 32) {
-      uint32_t r[32];
-      if (ws_row == nullptr) {
-        tmem_ld32(t_row + c, r);
-        tmem_ld_wait();
-      } else {
+// Epilogue of one 32-column chunk of one output row: r = the 32 fp32 accumulators of columns [n, n + 32).
+// ATTN_DO: the row is token (ab, as) of the joint sequence; dacc carries sum_d dO*O across the four 32-column chunks of a head,
+// so a thread must walk the chunks of a head in order.
+template <int EPI>
+__device__ __forceinline__ void epilogue_chunk(const GemmProb& q, const GemmParams& P, uint32_t* r, int row, bool row_ok, int n,
+                                               const bf16* gate_row, int ab, int as, float& dacc) {
+  uint32_t o[16];
+  uint4 bias4[4];
+  if (q.bias != nullptr) {
 #pragma unroll
-        for (int v = 0; v < 8; ++v) {
-          const float4 f = __ldcg(reinterpret_cast<const float4*>(ws_row + c) + v);  // written by other SMs' reds: read at L2
-          r[4 * v] = __float_as_uint(f.x); r[4 * v + 1] = __float_as_uint(f.y);
-          r[4 * v + 2] = __float_as_uint(f.z); r[4 * v + 3] = __float_as_uint(f.w);
-        }
-      }
-      const int n = n0 + c;
-      uint32_t o[16];
-      uint4 bias4[4];
-      if (q.bias != nullptr) {
+  for (int v = 0; v < 4; ++v) bias4[v] = __ldg(reinterpret_cast<const uint4*>(q.bias + n) + v);
+  } else {
 #pragma unroll
-        for (int v = 0; v < 4; ++v) bias4[v] = __ldg(reinterpret_cast<const uint4*>(q.bias + n) + v);
-      } else {
+  for (int v = 0; v < 4; ++v) bias4[v] = make_uint4(0, 0, 0, 0);
+  }
+  const uint32_t* bw = reinterpret_cast<const uint32_t*>(bias4);
+  if (EPI == QFX_EPI_BIAS) {
 #pragma unroll
-        for (int v = 0; v < 4; ++v) bias4[v] = make_uint4(0, 0, 0, 0);
-      }
-      const uint32_t* bw = reinterpret_cast<const uint32_t*>(bias4);
-      if (EPI == QFX_EPI_BIAS) {
+  for (int i = 0; i < 16; ++i) {
+    float v0 = __uint_as_float(r[2 * i]) * P.alpha + bf16_lo(bw[i]);
+    float v1 = __uint_as_float(r[2 * i + 1]) * P.alpha + bf16_hi(bw[i]);
+    o[i] = pack_bf16(v0, v1);
+  }
+  } else if (EPI == QFX_EPI_GELU) {
+  uint32_t u[16];
 #pragma unroll
-        for (int i = 0; i < 16; ++i) {
-          float v0 = __uint_as_float(r[2 * i]) * P.alpha + bf16_lo(bw[i]);
-          float v1 = __uint_as_float(r[2 * i + 1]) * P.alpha + bf16_hi(bw[i]);
-          o[i] = pack_bf16(v0, v1);
-        }
-      } else if (EPI == QFX_EPI_GELU) {
-        uint32_t u[16];
+  for (int i = 0; i < 16; ++i) {
+    u[i] = pack_bf16(__uint_as_float(r[2 * i]) + bf16_lo(bw[i]), __uint_as_float(r[2 * i + 1]) + bf16_hi(bw[i]));
+    o[i] = pack_bf16(gelu_tanh(bf16_lo(u[i])), gelu_tanh(bf16_hi(u[i])));
+  }
+  if (row_ok) {
+    uint4* dst2 = reinterpret_cast<uint4*>(q.out2 + (int64_t)row * q.ldo2 + n);
 #pragma unroll
-        for (int i = 0; i < 16; ++i) {
-          u[i] = pack_bf16(__uint_as_float(r[2 * i]) + bf16_lo(bw[i]), __uint_as_float(r[2 * i + 1]) + bf16_hi(bw[i]));
-          o[i] = pack_bf16(gelu_tanh(bf16_lo(u[i])), gelu_tanh(bf16_hi(u[i])));
-        }
-        if (row_ok) {
-          uint4* dst2 = reinterpret_cast<uint4*>(q.out2 + (int64_t)row * q.ldo2 + n);
+    for (int v = 0; v < 4; ++v) st_out(dst2 + v, make_uint4(u[4 * v], u[4 * v + 1], u[4 * v + 2], u[4 * v + 3]), P.stream_out);
+  }
+  } else if (EPI == QFX_EPI_RESID_GATE) {
+  if (row_ok) {
+    const uint4* rs = reinterpret_cast<const uint4*>(q.resid + (int64_t)row * q.ldr + n);
+    const uint4* gs = reinterpret_cast<const uint4*>(gate_row + n);
 #pragma unroll
-          for (int v = 0; v < 4; ++v) st_out(dst2 + v, make_uint4(u[4 * v], u[4 * v + 1], u[4 * v + 2], u[4 * v + 3]), P.stream_out);
-        }
-      } else if (EPI == QFX_EPI_RESID_GATE) {
-        if (row_ok) {
-          const uint4* rs = reinterpret_cast<const uint4*>(q.resid + (int64_t)row * q.ldr + n);
-          const uint4* gs = reinterpret_cast<const uint4*>(gate_row + n);
+    for (int v = 0; v < 4; ++v) {
+      uint4 rr = rs[v];
+      uint4 gg = __ldg(gs + v);
+      const uint32_t* rw = reinterpret_cast<const uint32_t*>(&rr);
+      const uint32_t* gw = reinterpret_cast<const uint32_t*>(&gg);
 #pragma unroll
-          for (int v = 0; v < 4; ++v) {
-            uint4 rr = rs[v];
-            uint4 gg = __ldg(gs + v);
-            const uint32_t* rw = reinterpret_cast<const uint32_t*>(&rr);
-            const uint32_t* gw = reinterpret_cast<const uint32_t*>(&gg);
-#pragma unroll
-            for (int e = 0; e < 4; ++e) {
-              const int i = 4 * v + e;
-              // eager bf16 rounding points of the reference: y=Linear(x) -> gate*y -> resid + (.)
-              float y0 = round_bf16(__uint_as_float(r[2 * i]) + bf16_lo(bw[i]));
-              float y1 = round_bf16(__uint_as_float(r[2 * i + 1]) + bf16_hi(bw[i]));
-              float z0 = round_bf16(bf16_lo(gw[e]) * y0);
-              float z1 = round_bf16(bf16_hi(gw[e]) * y1);
-              o[i] = pack_bf16(bf16_lo(rw[e]) + z0, bf16_hi(rw[e]) + z1);
-              if (q.out2 != nullptr) r[i] = pack_bf16(y0, y1);  // un-gated branch output (the accumulator registers are dead now)
-            }
-          }
-          if (q.out2 != nullptr) {  // kept when the gate's AdaLN linear carries LoRA: d gate = sum_t dOut * y
-            uint4* dst2 = reinterpret_cast<uint4*>(q.out2 + (int64_t)row * q.ldo2 + n);
-#pragma unroll
-            for (int v = 0; v < 4; ++v) dst2[v] = make_uint4(r[4 * v], r[4 * v + 1], r[4 * v + 2], r[4 * v + 3]);
-          }
-        }
-      } else if (EPI == QFX_EPI_ADD) {
-        if (row_ok) {
-          const uint4* rs = reinterpret_cast<const uint4*>(q.resid + (int64_t)row * q.ldr + n);
-#pragma unroll
-          for (int v = 0; v < 4; ++v) {
-            uint4 rr = rs[v];
-            const uint32_t* rw = reinterpret_cast<const uint32_t*>(&rr);
-#pragma unroll
-            for (int e = 0; e < 4; ++e) {
-              const int i = 4 * v + e;
-              o[i] = pack_bf16(bf16_lo(rw[e]) + round_bf16(__uint_as_float(r[2 * i]) * P.alpha),
-                               bf16_hi(rw[e]) + round_bf16(__uint_as_float(r[2 * i + 1]) * P.alpha));
-            }
-          }
-        }
-      } else if (EPI == QFX_EPI_ATTN_DO) {
-        if (row_ok) {
-          const uint4* os = reinterpret_cast<const uint4*>(q.aux + (int64_t)row * q.ldaux + n);
-#pragma unroll
-          for (int v = 0; v < 4; ++v) {
-            uint4 oo = os[v];
-            const uint32_t* ow = reinterpret_cast<const uint32_t*>(&oo);
-#pragma unroll
-            for (int e = 0; e < 4; ++e) {
-              const int i = 4 * v + e;
-              const float g0 = round_bf16(__uint_as_float(r[2 * i]) * P.alpha), g1 = round_bf16(__uint_as_float(r[2 * i + 1]) * P.alpha);
-              o[i] = pack_bf16(g0, g1);
-              dacc += g0 * bf16_lo(ow[e]) + g1 * bf16_hi(ow[e]);
-            }
-          }
-          const int h = n >> 7, cc = n & 127;
-          const int64_t pos = ((int64_t)ab * P.attn_H + h) * P.attn_S + as;
-          uint4* dj = reinterpret_cast<uint4*>(q.out + pos * 128 + cc);
-#pragma unroll
-          for (int v = 0; v < 4; ++v) dj[v] = make_uint4(o[4 * v], o[4 * v + 1], o[4 * v + 2], o[4 * v + 3]);
-          if (cc == 96) {  // last chunk of this head
-            P.delta[pos] = dacc;
-            dacc = 0.f;
-          }
-          if (q.out2 != nullptr) {
-            uint4* dst2 = reinterpret_cast<uint4*>(q.out2 + (int64_t)row * q.ldo2 + n);
-#pragma unroll
-            for (int v = 0; v < 4; ++v) dst2[v] = make_uint4(o[4 * v], o[4 * v + 1], o[4 * v + 2], o[4 * v + 3]);
-          }
-        }
-      } else if (EPI == QFX_EPI_DGELU) {
-        if (row_ok) {
-          const uint4* us = reinterpret_cast<const uint4*>(q.aux + (int64_t)row * q.ldaux + n);
-#pragma unroll
-          for (int v = 0; v < 4; ++v) {
-            uint4 uu = us[v];
-            const uint32_t* uw = reinterpret_cast<const uint32_t*>(&uu);
-#pragma unroll
-            for (int e = 0; e < 4; ++e) {
-              const int i = 4 * v + e;
-              float g0 = round_bf16(__uint_as_float(r[2 * i]) * P.alpha);
-              float g1 = round_bf16(__uint_as_float(r[2 * i + 1]) * P.alpha);
-              o[i] = pack_bf16(g0 * gelu_tanh_grad(bf16_lo(uw[e])), g1 * gelu_tanh_grad(bf16_hi(uw[e])));
-            }
-          }
-        }
-      }
-      if (row_ok && EPI != QFX_EPI_ATTN_DO) {
-        uint4* dst = reinterpret_cast<uint4*>(q.out + (int64_t)row * q.ldo + n);
-#pragma unroll
-        for (int v = 0; v < 4; ++v) st_out(dst + v, make_uint4(o[4 * v], o[4 * v + 1], o[4 * v + 2], o[4 * v + 3]), P.stream_out);
+      for (int e = 0; e < 4; ++e) {
+        const int i = 4 * v + e;
+        // eager bf16 rounding points of the reference: y=Linear(x) -> gate*y -> resid + (.)
+        float y0 = round_bf16(__uint_as_float(r[2 * i]) + bf16_lo(bw[i]));
+        float y1 = round_bf16(__uint_as_float(r[2 * i + 1]) + bf16_hi(bw[i]));
+        float z0 = round_bf16(bf16_lo(gw[e]) * y0);
+        float z1 = round_bf16(bf16_hi(gw[e]) * y1);
+        o[i] = pack_bf16(bf16_lo(rw[e]) + z0, bf16_hi(rw[e]) + z1);
+        if (q.out2 != nullptr) r[i] = pack_bf16(y0, y1);  // un-gated branch output (the accumulator registers are dead now)
       }
     }
+    if (q.out2 != nullptr) {  // kept when the gate's AdaLN linear carries LoRA: d gate = sum_t dOut * y
+      uint4* dst2 = reinterpret_cast<uint4*>(q.out2 + (int64_t)row * q.ldo2 + n);
+#pragma unroll
+      for (int v = 0; v < 4; ++v) dst2[v] = make_uint4(r[4 * v], r[4 * v + 1], r[4 * v + 2], r[4 * v + 3]);
+    }
+  }
+  } else if (EPI == QFX_EPI_ADD) {
+  if (row_ok) {
+    const uint4* rs = reinterpret_cast<const uint4*>(q.resid + (int64_t)row * q.ldr + n);
+#pragma unroll
+    for (int v = 0; v < 4; ++v) {
+      uint4 rr = rs[v];
+      const uint32_t* rw = reinterpret_cast<const uint32_t*>(&rr);
+#pragma unroll
+      for (int e = 0; e < 4; ++e) {
+        const int i = 4 * v + e;
+        o[i] = pack_bf16(bf16_lo(rw[e]) + round_bf16(__uint_as_float(r[2 * i]) * P.alpha),
+                         bf16_hi(rw[e]) + round_bf16(__uint_as_float(r[2 * i + 1]) * P.alpha));
+      }
+    }
+  }
+  } else if (EPI == QFX_EPI_ATTN_DO) {
+  if (row_ok) {
+    const uint4* os = reinterpret_cast<const uint4*>(q.aux + (int64_t)row * q.ldaux + n);
+#pragma unroll
+    for (int v = 0; v < 4; ++v) {
+      uint4 oo = os[v];
+      const uint32_t* ow = reinterpret_cast<const uint32_t*>(&oo);
+#pragma unroll
+      for (int e = 0; e < 4; ++e) {
+        const int i = 4 * v + e;
+        const float g0 = round_bf16(__uint_as_float(r[2 * i]) * P.alpha), g1 = round_bf16(__uint_as_float(r[2 * i + 1]) * P.alpha);
+        o[i] = pack_bf16(g0, g1);
+        dacc += g0 * bf16_lo(ow[e]) + g1 * bf16_hi(ow[e]);
+      }
+    }
+    const int h = n >> 7, cc = n & 127;
+    const int64_t pos = ((int64_t)ab * P.attn_H + h) * P.attn_S + as;
+    uint4* dj = reinterpret_cast<uint4*>(q.out + pos * 128 + cc);
+#pragma unroll
+    for (int v = 0; v < 4; ++v) dj[v] = make_uint4(o[4 * v], o[4 * v + 1], o[4 * v + 2], o[4 * v + 3]);
+    if (cc == 96) {  // last chunk of this head
+      P.delta[pos] = dacc;
+      dacc = 0.f;
+    }
+    if (q.out2 != nullptr) {
+      uint4* dst2 = reinterpret_cast<uint4*>(q.out2 + (int64_t)row * q.ldo2 + n);
+#pragma unroll
+      for (int v = 0; v < 4; ++v) dst2[v] = make_uint4(o[4 * v], o[4 * v + 1], o[4 * v + 2], o[4 * v + 3]);
+    }
+  }
+  } else if (EPI == QFX_EPI_DGELU) {
+  if (row_ok) {
+    const uint4* us = reinterpret_cast<const uint4*>(q.aux + (int64_t)row * q.ldaux + n);
+#pragma unroll
+    for (int v = 0; v < 4; ++v) {
+      uint4 uu = us[v];
+      const uint32_t* uw = reinterpret_cast<const uint32_t*>(&uu);
+#pragma unroll
+      for (int e = 0; e < 4; ++e) {
+        const int i = 4 * v + e;
+        float g0 = round_bf16(__uint_as_float(r[2 * i]) * P.alpha);
+        float g1 = round_bf16(__uint_as_float(r[2 * i + 1]) * P.alpha);
+        o[i] = pack_bf16(g0 * gelu_tanh_grad(bf16_lo(uw[e])), g1 * gelu_tanh_grad(bf16_hi(uw[e])));
+      }
+    }
+  }
+  }
+  if (row_ok && EPI != QFX_EPI_ATTN_DO) {
+  uint4* dst = reinterpret_cast<uint4*>(q.out + (int64_t)row * q.ldo + n);
+#pragma unroll
+  for (int v = 0; v < 4; ++v) st_out(dst + v, make_uint4(o[4 * v], o[4 * v + 1], o[4 * v + 2], o[4 * v + 3]), P.stream_out);
+  }
+}
+
+template <int BN, int TB>
+__device__ __forceinline__ void wgmma_tile(float* d, uint64_t a, uint64_t b, int scale_d) {
+  if constexpr (BN == 64) wgmma_ss_n64<0, TB>(d, a, b, scale_d);
+  else if constexpr (BN == 128) wgmma_ss_n128<0, TB>(d, a, b, scale_d);
+  else if constexpr (BN == 192) wgmma_ss_n192<0, TB>(d, a, b, scale_d);
+  else wgmma_ss_n256<0, TB>(d, a, b, scale_d);
 }
 
 template <int BN, bool TRANS_B, int EPI>
-__global__ void __launch_bounds__(256, 1) gemm_kernel(const __grid_constant__ GemmParams P) {
+__global__ void __launch_bounds__(384, 1) gemm_kernel(const __grid_constant__ GemmParams P) {
   using C = GemmCfg<BN>;
   extern __shared__ uint8_t smem_raw[];
   const uint32_t smem_base = (smem_u32(smem_raw) + 1023u) & ~1023u;
-  const uint32_t bar_base = smem_base + C::STAGES * C::STAGE_BYTES;
+  uint8_t* smem_gen = smem_raw + (smem_base - smem_u32(smem_raw));
+  float* epi_stage = reinterpret_cast<float*>(smem_gen + C::STAGES * C::STAGE_BYTES);
+  const uint32_t bar_base = smem_base + C::STAGES * C::STAGE_BYTES + C::EPI_BYTES;
   auto full_bar = [&](int s) { return bar_base + 8u * s; };
   auto empty_bar = [&](int s) { return bar_base + 8u * (C::STAGES + s); };
-  auto tfull_bar = [&](int s) { return bar_base + 8u * (2 * C::STAGES + s); };
-  auto tempty_bar = [&](int s) { return bar_base + 8u * (2 * C::STAGES + 2 + s); };
-  const uint32_t tmem_slot = bar_base + 8u * (2 * C::STAGES + 4);
-  uint8_t* smem_gen = smem_raw + (smem_base - smem_u32(smem_raw));
 
-  const int warp = threadIdx.x >> 5;
-  const int lane = threadIdx.x & 31;
+  const int wg = threadIdx.x >> 7;
 
-  if (warp == 0 && lane == 0) {
-    for (int i = 0; i < P.nprob; ++i) {
-      tma_prefetch_desc(&P.p[i].tmA);
-      tma_prefetch_desc(&P.p[i].tmB);
-      if (P.p[i].kb2) {
-        tma_prefetch_desc(&P.p[i].tmA2);
-        tma_prefetch_desc(&P.p[i].tmB2);
-      }
-    }
-  }
-  if (warp == 1 && lane == 0) {
+  if (threadIdx.x == 0) {
     for (int s = 0; s < C::STAGES; ++s) {
       mbar_init(full_bar(s), 1);
-      mbar_init(empty_bar(s), 1);
-    }
-    for (int s = 0; s < 2; ++s) {
-      mbar_init(tfull_bar(s), 1);
-      mbar_init(tempty_bar(s), 4);
+      mbar_init(empty_bar(s), 8);  // lane 0 of each of the 8 consumer warps
     }
     fence_barrier_init();
   }
-  if (warp == 2) tmem_alloc(tmem_slot, C::TMEM_COLS);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *reinterpret_cast<volatile uint32_t*>(smem_gen + (tmem_slot - smem_base));
 
   const int nkb = P.K / BK;
 
@@ -283,9 +241,18 @@ __global__ void __launch_bounds__(256, 1) gemm_kernel(const __grid_constant__ Ge
     n0 = n_blk * BN;
   };
 
-  if (warp == 0) {
+  if (wg == 0) {
     // =============================================================== TMA producer
-    if (lane == 0) {
+    reg_dealloc<40>();  // one thread issues TMA: the consumers take its registers for the BN/2 accumulators + the epilogue
+    if (threadIdx.x == 0) {
+      for (int i = 0; i < P.nprob; ++i) {
+        tma_prefetch_desc(&P.p[i].tmA);
+        tma_prefetch_desc(&P.p[i].tmB);
+        if (P.p[i].kb2) {
+          tma_prefetch_desc(&P.p[i].tmA2);
+          tma_prefetch_desc(&P.p[i].tmB2);
+        }
+      }
       int stage = 0;
       uint32_t phase = 0;
       for (int tile = blockIdx.x; tile < P.total_tiles; tile += gridDim.x) {
@@ -321,298 +288,77 @@ __global__ void __launch_bounds__(256, 1) gemm_kernel(const __grid_constant__ Ge
         }
       }
     }
-  } else if (warp == 1) {
-    // =============================================================== MMA issuer
-    if (lane == 0) {
-      constexpr uint32_t idesc = idesc_bf16(BM, BN, 0, TRANS_B ? 1 : 0);
-      int stage = 0;
-      uint32_t phase = 0;
-      int it = 0;
-      for (int tile = blockIdx.x; tile < P.total_tiles; tile += gridDim.x, ++it) {
-        int prob, m0, n0;
-        decode(tile, prob, m0, n0);
-        const int kb_total = nkb + P.p[prob].kb2;
-        const int acc = it & 1;
-        const uint32_t acc_phase = (it >> 1) & 1;
-        mbar_wait(tempty_bar(acc), acc_phase ^ 1);
-        tc_fence_after();
-        const uint32_t d_tmem = tmem_base + acc * BN;
-        for (int kb = 0; kb < kb_total; ++kb) {
-          mbar_wait(full_bar(stage), phase);
-          tc_fence_after();
-          const uint32_t a_addr = smem_base + stage * C::STAGE_BYTES;
-          const uint32_t b_addr = a_addr + C::A_BYTES;
-#pragma unroll
-          for (int k = 0; k < BK / 16; ++k) {
-            const uint64_t ad = sdesc_sw128(a_addr + k * 32, 16, 1024);
-            const uint64_t bd = TRANS_B ? sdesc_sw128(b_addr + k * 2048, 8192, 1024) : sdesc_sw128(b_addr + k * 32, 16, 1024);
-            umma_bf16(d_tmem, ad, bd, idesc, (kb | k) != 0);
-          }
-          umma_commit(empty_bar(stage));
-          if (++stage == C::STAGES) { stage = 0; phase ^= 1; }
-        }
-        umma_commit(tfull_bar(acc));
-      }
-    }
-  } else if (warp >= 4) {
-    // =============================================================== epilogue
-    const int q4 = warp & 3;
-    int it = 0;
-    for (int tile = blockIdx.x; tile < P.total_tiles; tile += gridDim.x, ++it) {
+  } else {
+    // =============================================================== consumers: rows 64 * cw .. + 63 of each tile
+    reg_alloc<232>();  // 128 x 40 + 256 x 232 = 64512 <= the 65536 registers of the SM
+    const int cw = wg - 1;
+    const int t = threadIdx.x & 127, w = t >> 5, l = t & 31;
+    float* stg = epi_stage + cw * 64 * C::EPI_LD;
+    float acc[BN / 2];
+    int stage = 0;
+    uint32_t phase = 0;
+    for (int tile = blockIdx.x; tile < P.total_tiles; tile += gridDim.x) {
       int prob, m0, n0;
       decode(tile, prob, m0, n0);
       const GemmProb& q = P.p[prob];
-      const int acc = it & 1;
-      const uint32_t acc_phase = (it >> 1) & 1;
-      mbar_wait(tfull_bar(acc), acc_phase);
-      tc_fence_after();
-      const int row = m0 + q4 * 32 + lane;
-      const bool row_ok = row < q.M;
-      const uint32_t t_row = tmem_base + ((uint32_t)(q4 * 32) << 16) + acc * BN;
-      epilogue_tile<BN, EPI>(q, P, t_row, row, row_ok, n0);
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(tempty_bar(acc));
-    }
-  }
-
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 2) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, C::TMEM_COLS);
-  }
-}
-
-// =====================================================================================================================
-// 2-CTA variant (cta_group::2): a CTA pair on one TPC computes a 256 x BN tile.  Each CTA stages its own 128 rows of A and
-// HALF of the B tile, so per-SM shared-memory traffic drops by a third and the ring holds 6 stages instead of 4 for the
-// same 192 KB; the leader CTA issues tcgen05.mma.cta_group::2 (M = 256), completion is multicast to both CTAs' barriers.
-// floats of padding per split-K workspace row: with a power-of-two row stride (1024 B) the row-per-thread reads of the final
-// epilogue camp on a few L2 slices (measured: +40 us per GEMM)
-constexpr int WS_PAD = 8;
-template <int BN>
-struct Gemm2Cfg {
-  static constexpr int A_BYTES = BM * BK * 2;
-  static constexpr int B_BYTES = (BN / 2) * BK * 2;  // this CTA's half of the B tile
-  static constexpr int STAGE_BYTES = A_BYTES + B_BYTES;
-  static constexpr int STAGES = BN == 256 ? 6 : 8;
-  static constexpr int TMEM_COLS = 2 * BN <= 256 ? 256 : 512;
-  static constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + 1024 + 256;
-};
-
-template <int BN, bool TRANS_B, int EPI>
-__global__ void __cluster_dims__(2, 1, 1) __launch_bounds__(256, 1) gemm2_kernel(const __grid_constant__ GemmParams P) {
-  using C = Gemm2Cfg<BN>;
-  extern __shared__ uint8_t smem_raw[];
-  const uint32_t smem_base = (smem_u32(smem_raw) + 1023u) & ~1023u;
-  const uint32_t bar_base = smem_base + C::STAGES * C::STAGE_BYTES;
-  auto full_bar = [&](int s) { return bar_base + 8u * s; };
-  auto empty_bar = [&](int s) { return bar_base + 8u * (C::STAGES + s); };
-  auto tfull_bar = [&](int s) { return bar_base + 8u * (2 * C::STAGES + s); };
-  auto tempty_bar = [&](int s) { return bar_base + 8u * (2 * C::STAGES + 2 + s); };
-  const uint32_t tmem_slot = bar_base + 8u * (2 * C::STAGES + 4);
-  uint8_t* smem_gen = smem_raw + (smem_base - smem_u32(smem_raw));
-
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const uint32_t rank = cluster_ctarank();
-  const bool leader = rank == 0;
-  const int cluster_id = blockIdx.x >> 1, n_clusters = gridDim.x >> 1;
-
-  if (warp == 1 && lane == 0) {
-    for (int s = 0; s < C::STAGES; ++s) {
-      mbar_init(full_bar(s), 1);   // leader's arrive.expect_tx covers the bytes of BOTH CTAs (the peer only adds complete_tx)
-      mbar_init(empty_bar(s), 1);  // multicast tcgen05.commit
-    }
-    for (int s = 0; s < 2; ++s) {
-      mbar_init(tfull_bar(s), 1);   // multicast tcgen05.commit
-      mbar_init(tempty_bar(s), 8);  // leader: 4 epilogue warps of each CTA
-    }
-    fence_barrier_init();
-  }
-  if (warp == 2) tmem_alloc_2sm(tmem_slot, C::TMEM_COLS);
-  tc_fence_before();
-  cluster_sync_all();
-  tc_fence_after();
-  const uint32_t tmem_base = *reinterpret_cast<volatile uint32_t*>(smem_gen + (tmem_slot - smem_base));
-
-  const int nkb = P.K / BK;
-  auto decode = [&](int tile, int& prob, int& m0, int& n0) {  // tiles are 256 rows tall here
-    int n_blk, mm;
-    if (P.n_fast) {
-      mm = tile / P.tiles_n;
-      n_blk = tile - mm * P.tiles_n;
-    } else {
-      n_blk = tile / P.tiles_m_total;
-      mm = tile - n_blk * P.tiles_m_total;
-    }
-    prob = 0;
+      const int kb_total = nkb + q.kb2;
+      int prev = 0;
+      reg_fence(acc, BN / 2);
+      for (int kb = 0; kb < kb_total; ++kb) {
+        mbar_wait(full_bar(stage), phase);
+        const uint32_t a_addr = smem_base + stage * C::STAGE_BYTES + cw * 64 * 128;
+        const uint32_t b_addr = smem_base + stage * C::STAGE_BYTES + C::A_BYTES;
+        wgmma_fence();
 #pragma unroll
-    for (int i = 0; i < QFX_MAX_PROBLEMS - 1; ++i) prob += (i + 1 < P.nprob && mm >= P.tiles_m_end[i]) ? 1 : 0;
-    const int local = prob ? mm - P.tiles_m_end[prob - 1] : mm;
-    const int* rt = P.p[prob].row_tiles;
-    m0 = (rt ? __ldg(rt + local) : local * 256) + (int)rank * BM;
-    n0 = n_blk * BN;
-  };
-  // Work units of this CTA pair, in order: whole tiles cluster_id, cluster_id + n_clusters, ... below tail_first, then (split-K of
-  // the last partial wave) at most ONE K range of a tail tile.  All three roles walk the same list.
-  struct Unit {
-    int tile, kb_lo, kb_hi;
-    bool lora, split;
-  };
-  auto unit_at = [&](int i, Unit& u) -> bool {
-    const int tile = cluster_id + i * n_clusters;
-    if (tile < P.tail_first) {
-      u.tile = tile; u.kb_lo = 0; u.kb_hi = nkb; u.lora = true; u.split = false;
-      return true;
-    }
-    const int idx = tile - P.tail_first, R = P.total_tiles - P.tail_first;
-    if (P.tail_split <= 1 || idx >= R * P.tail_split) return false;
-    const int part = idx / R;
-    u.tile = P.tail_first + idx - part * R;
-    u.kb_lo = part * nkb / P.tail_split;
-    u.kb_hi = (part + 1) * nkb / P.tail_split;
-    u.lora = part == P.tail_split - 1;  // the LoRA k-blocks ride with the last K range
-    u.split = true;
-    return true;
-  };
-  __shared__ int tail_last;
-
-  if (warp == 0) {
-    // =============================================================== TMA producer (both CTAs)
-    if (lane == 0) {
-      int stage = 0;
-      uint32_t phase = 0;
-      Unit u;
-      for (int i = 0; unit_at(i, u); ++i) {
-        int prob, m0, n0;
-        decode(u.tile, prob, m0, n0);
-        const GemmProb& q = P.p[prob];
-        const int kb_end = u.lora ? nkb + q.kb2 : nkb;  // kb in [kb_lo, kb_hi) are base k-blocks, [nkb, kb_end) the LoRA ones
-        const int grp = (!TRANS_B && P.lora_group_n > 0) ? n0 / P.lora_group_n : 0;
-        const int nh = n0 + (int)rank * (BN / 2);  // this CTA's half of the B columns
-        for (int kb = u.kb_lo; kb < kb_end; kb = (kb + 1 == u.kb_hi ? nkb : kb + 1)) {
-          mbar_wait(empty_bar(stage), phase ^ 1);
-          const uint32_t a_dst = smem_base + stage * C::STAGE_BYTES;
-          const uint32_t b_dst = a_dst + C::A_BYTES;
-          const uint32_t fb = full_bar(stage);
-          if (leader) mbar_expect_tx(fb, 2 * C::STAGE_BYTES);
-          if (kb < nkb) {
-            tma_load_2d_2sm(a_dst, &q.tmA, fb, kb * BK, m0);
-            if (!TRANS_B) {
-              tma_load_2d_2sm(b_dst, &q.tmB, fb, kb * BK, nh);
-            } else {
-#pragma unroll
-              for (int a = 0; a < BN / 128; ++a) tma_load_2d_2sm(b_dst + a * 8192, &q.tmB, fb, nh + a * 64, kb * BK);
-            }
-          } else {
-            const int j = kb - nkb;
-            tma_load_2d_2sm(a_dst, &q.tmA2, fb, q.a2_col0 + (grp * q.kb2 + j) * 64, m0);
-            if (!TRANS_B) {
-              tma_load_2d_2sm(b_dst, &q.tmB2, fb, j * 64, nh);
-            } else {
-#pragma unroll
-              for (int a = 0; a < BN / 128; ++a) tma_load_2d_2sm(b_dst + a * 8192, &q.tmB2, fb, nh + a * 64, j * 64);
-            }
-          }
-          if (++stage == C::STAGES) { stage = 0; phase ^= 1; }
+        for (int k = 0; k < BK / 16; ++k) {
+          const uint64_t ad = sdesc_sw128(a_addr + k * 32, 16, 1024);
+          const uint64_t bd = TRANS_B ? sdesc_sw128(b_addr + k * 2048, 8192, 1024) : sdesc_sw128(b_addr + k * 32, 16, 1024);
+          wgmma_tile<BN, TRANS_B ? 1 : 0>(acc, ad, bd, (kb | k) != 0);
         }
-      }
-    }
-  } else if (warp == 1) {
-    // =============================================================== MMA issuer (leader CTA only)
-    if (lane == 0 && leader) {
-      constexpr uint32_t idesc = idesc_bf16(256, BN, 0, TRANS_B ? 1 : 0);
-      int stage = 0;
-      uint32_t phase = 0;
-      Unit u;
-      for (int it = 0; unit_at(it, u); ++it) {
-        int prob, m0, n0;
-        decode(u.tile, prob, m0, n0);
-        const int kb_total = (u.kb_hi - u.kb_lo) + (u.lora ? P.p[prob].kb2 : 0);
-        const int acc = it & 1;
-        const uint32_t acc_phase = (it >> 1) & 1;
-        mbar_wait(tempty_bar(acc), acc_phase ^ 1);
-        tc_fence_after();
-        const uint32_t d_tmem = tmem_base + acc * BN;
-        for (int kb = 0; kb < kb_total; ++kb) {
-          mbar_wait(full_bar(stage), phase);
-          tc_fence_after();
-          const uint32_t a_addr = smem_base + stage * C::STAGE_BYTES;
-          const uint32_t b_addr = a_addr + C::A_BYTES;
-#pragma unroll
-          for (int k = 0; k < BK / 16; ++k) {
-            const uint64_t ad = sdesc_sw128(a_addr + k * 32, 16, 1024);
-            const uint64_t bd = TRANS_B ? sdesc_sw128(b_addr + k * 2048, 8192, 1024) : sdesc_sw128(b_addr + k * 32, 16, 1024);
-            umma_bf16_2sm(d_tmem, ad, bd, idesc, (kb | k) != 0);
-          }
-          umma_commit_2sm(empty_bar(stage), 3);
-          if (++stage == C::STAGES) { stage = 0; phase ^= 1; }
+        wgmma_commit();
+        if (kb > 0) {  // the k-block before this one has been consumed: its stage goes back to the producer
+          wgmma_wait<1>();
+          if (l == 0) mbar_arrive(empty_bar(prev));
         }
-        umma_commit_2sm(tfull_bar(acc), 3);
+        prev = stage;
+        if (++stage == C::STAGES) { stage = 0; phase ^= 1; }
       }
-    }
-  } else if (warp >= 4) {
-    // =============================================================== epilogue (both CTAs, own 128 rows)
-    const int q4 = warp & 3;
-    Unit u;
-    for (int it = 0; unit_at(it, u); ++it) {
-      int prob, m0, n0;
-      decode(u.tile, prob, m0, n0);
-      const GemmProb& q = P.p[prob];
-      const int acc = it & 1;
-      const uint32_t acc_phase = (it >> 1) & 1;
-      mbar_wait(tfull_bar(acc), acc_phase);
-      tc_fence_after();
-      const int row = m0 + q4 * 32 + lane;
-      const bool row_ok = row < q.M;
-      const uint32_t t_row = tmem_base + ((uint32_t)(q4 * 32) << 16) + acc * BN;
-      float* ws_row = nullptr;
-      if (!u.split) {
-        epilogue_tile<BN, EPI>(q, P, t_row, row, row_ok, n0);
-      } else {  // partial sum over [kb_lo, kb_hi): add it into the workspace row of this (tile, CTA half)
-        const int slot = (u.tile - P.tail_first) * 2 + (int)rank;
-        ws_row = P.tail_ws + ((int64_t)slot * BM + q4 * 32 + lane) * (BN + WS_PAD);  // padded rows: a power-of-two row stride camps on L2 slices
-#pragma unroll 1
-        for (int c = 0; c < BN; c += 32) {
+      wgmma_wait<0>();
+      reg_fence(acc, BN / 2);
+      if (l == 0) mbar_arrive(empty_bar(prev));
+
+      // ---- epilogue: 32-column chunks staged through shared memory so that thread t < 64 owns output row t of the warpgroup
+      const int row = m0 + cw * 64 + t;
+      const bool row_ok = t < 64 && row < q.M;
+      const bf16* gate_row = nullptr;
+      if (EPI == QFX_EPI_RESID_GATE && row_ok) gate_row = q.gate + (int64_t)(row / q.rows_per_batch) * q.ldg;
+      int ab = 0, as = 0;
+      float dacc = 0.f;
+      if (EPI == QFX_EPI_ATTN_DO) {
+        ab = row / q.rows_per_batch;
+        as = q.s_offset + row - ab * q.rows_per_batch;
+      }
+#pragma unroll
+      for (int c = 0; c < BN; c += 32) {
+#pragma unroll
+        for (int jj = 0; jj < 4; ++jj) {
+          const int j = c / 8 + jj;
+          const int r0 = 16 * w + (l >> 2), cc = jj * 8 + 2 * (l & 3);
+          stg[r0 * C::EPI_LD + cc] = acc[4 * j];
+          stg[r0 * C::EPI_LD + cc + 1] = acc[4 * j + 1];
+          stg[(r0 + 8) * C::EPI_LD + cc] = acc[4 * j + 2];
+          stg[(r0 + 8) * C::EPI_LD + cc + 1] = acc[4 * j + 3];
+        }
+        named_bar(1 + cw, 128);
+        if (t < 64) {
           uint32_t r[32];
-          tmem_ld32(t_row + c, r);
-          tmem_ld_wait();
 #pragma unroll
-          for (int v = 0; v < 8; ++v) red_add_v4(ws_row + c + 4 * v, r[4 * v], r[4 * v + 1], r[4 * v + 2], r[4 * v + 3]);
+          for (int i = 0; i < 32; ++i) r[i] = __float_as_uint(stg[t * C::EPI_LD + i]);
+          epilogue_chunk<EPI>(q, P, r, row, row_ok, n0 + c, gate_row, ab, as, dacc);
         }
-      }
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) {
-        if (leader) mbar_arrive(tempty_bar(acc));
-        else mbar_arrive_remote(tempty_bar(acc), 0);
-      }
-      if (u.split) {
-        // the CTA whose arrival completes the count owns the epilogue of this half tile (threadfence + counter pattern)
-        const int slot = (u.tile - P.tail_first) * 2 + (int)rank;
-        __threadfence();
-        asm volatile("bar.sync 1, 128;" ::: "memory");
-        if (threadIdx.x == 128) {
-          const int old = atomicAdd(P.tail_cnt + slot, 1);
-          tail_last = old == P.tail_split - 1;
-          if (tail_last) P.tail_cnt[slot] = 0;  // ready for the next launch
-        }
-        asm volatile("bar.sync 1, 128;" ::: "memory");
-        if (tail_last) {
-          __threadfence();
-          epilogue_tile<BN, EPI>(q, P, 0u, row, row_ok, n0, ws_row);
-        }
-        asm volatile("bar.sync 1, 128;" ::: "memory");  // tail_last is re-used only after everyone has read it
+        named_bar(1 + cw, 128);
       }
     }
-  }
-
-  tc_fence_before();
-  cluster_sync_all();
-  if (warp == 2) {
-    tc_fence_after();
-    tmem_dealloc_2sm(tmem_base, C::TMEM_COLS);
   }
 }
 
@@ -637,106 +383,9 @@ static int launch(const GemmParams& P, cudaStream_t stream) {
     attr_done[dev & 63] = true;
   }
   int grid = P.total_tiles < num_sms() ? P.total_tiles : num_sms();
-  kern<<<grid, 256, C::SMEM_BYTES, stream>>>(P);
+  kern<<<grid, 384, C::SMEM_BYTES, stream>>>(P);
   QFX_CUDA(cudaGetLastError());
   return 0;
-}
-
-// Split-K scratch of the CTA-pair kernel: ONE workspace + arrival counters per device, shared by every template instantiation,
-// allocated on the first launch that needs it on that device (the only allocation this library makes after load; it happens during
-// the eager warm-up step, never inside a captured graph).  GEMMs of one device are issued from one stream at a time (include/qfx.h).
-static int tail_workspace(float** ws, int** cnt) {
-  constexpr int MAX_DEV = 64;
-  static float* g_ws[MAX_DEV] = {};
-  static int* g_cnt[MAX_DEV] = {};
-  int dev = 0;
-  QFX_CUDA(cudaGetDevice(&dev));
-  if (dev < 0 || dev >= MAX_DEV) {
-    set_error("qfx_gemm_bf16: device ordinal %d out of range", dev);
-    return -1;
-  }
-  if (g_ws[dev] == nullptr) {
-    const size_t bytes = (size_t)(num_sms() / 2) * 256 * (256 + WS_PAD) * sizeof(float);
-    QFX_CUDA(cudaMalloc(&g_ws[dev], bytes));
-    QFX_CUDA(cudaMemset(g_ws[dev], 0, bytes));
-    QFX_CUDA(cudaMalloc(&g_cnt[dev], num_sms() * sizeof(int)));
-    QFX_CUDA(cudaMemset(g_cnt[dev], 0, num_sms() * sizeof(int)));
-  }
-  *ws = g_ws[dev];
-  *cnt = g_cnt[dev];
-  return 0;
-}
-
-template <int BN, bool TRANS_B, int EPI>
-static int launch2(const GemmParams& P, cudaStream_t stream) {
-  using C = Gemm2Cfg<BN>;
-  auto kern = gemm2_kernel<BN, TRANS_B, EPI>;
-  static bool attr_done[64] = {};  // function attributes are per device
-  int dev = 0;
-  QFX_CUDA(cudaGetDevice(&dev));
-  if (!attr_done[dev & 63]) {
-    QFX_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, C::SMEM_BYTES));
-    attr_done[dev & 63] = true;
-  }
-  int clusters = num_sms() / 2;
-  if (P.total_tiles < clusters) clusters = P.total_tiles;
-  GemmParams Q = P;
-  Q.tail_first = P.total_tiles;
-  Q.tail_split = 1;
-  // Tile order.  M-first re-reads all of A once per wave of N blocks: fine while A (rows x K) stays in the 126 MB L2, but for the
-  // K = 3D / 4D contractions A is 177-236 MB and ncu showed 1.8 GB of DRAM reads for 0.39 GB of operands.  N-first keeps a few
-  // row blocks of A resident and re-reads the (per-stream 57-75 MB) weight instead.
-  {
-    double a_bytes = 0;
-    for (int i = 0; i < P.nprob; ++i) a_bytes += 2.0 * P.p[i].M * P.K;
-    const double w_bytes = 2.0 * P.N * P.K;  // per stream
-    static const int force = getenv("QFX_GEMM_NFAST") ? atoi(getenv("QFX_GEMM_NFAST")) : -1;
-    Q.n_fast = force >= 0 ? force : (a_bytes > 96e6 && w_bytes < 96e6);
-  }
-  // Split-K of the last partial wave: R leftover tiles leave clusters - R pairs idle for a whole tile time; with long K (the
-  // D<->4D and 3D->D contractions) each leftover tile is cut into floor(clusters / R) K ranges instead.  QFX_GEMM_NO_SPLITK=1
-  // disables it (A/B).  The workspace is process-wide: GEMMs are issued from one stream at a time.
-  static const bool no_split = getenv("QFX_GEMM_NO_SPLITK") != nullptr;
-  const int nkb = P.K / BK, R = P.total_tiles % clusters;
-  static const int min_kb = getenv("QFX_GEMM_SPLITK_MIN_KB") ? atoi(getenv("QFX_GEMM_SPLITK_MIN_KB")) : 64;  // A/B: 48 lets K = 3072 split too
-  if (!no_split && P.total_tiles > clusters && R > 0 && nkb >= min_kb) {
-    int S = clusters / R;
-    if (S > nkb / 8) S = nkb / 8;  // at least 8 k-blocks per range
-    if (S >= 2) {
-      float* ws = nullptr;
-      int* cnt = nullptr;
-      if (tail_workspace(&ws, &cnt)) return -1;
-      // (zeroing the rows inside the kernel after the final read was measured at ~100 us per GEMM; a memset of the 3 MB in use is ~2)
-      QFX_CUDA(cudaMemsetAsync(ws, 0, (size_t)R * 256 * (BN + WS_PAD) * sizeof(float), stream));
-      Q.tail_first = P.total_tiles - R;
-      Q.tail_split = S;
-      Q.tail_ws = ws;
-      Q.tail_cnt = cnt;
-    }
-  }
-  kern<<<2 * clusters, 256, C::SMEM_BYTES, stream>>>(Q);
-  QFX_CUDA(cudaGetLastError());
-  return 0;
-}
-
-template <int BN>
-static int dispatch2(const GemmParams& P, int trans_b, int epi, cudaStream_t s) {
-  if (!trans_b) {
-    switch (epi) {
-      case QFX_EPI_BIAS: return launch2<BN, false, QFX_EPI_BIAS>(P, s);
-      case QFX_EPI_GELU: return launch2<BN, false, QFX_EPI_GELU>(P, s);
-      case QFX_EPI_RESID_GATE: return launch2<BN, false, QFX_EPI_RESID_GATE>(P, s);
-    }
-  } else {
-    switch (epi) {
-      case QFX_EPI_BIAS: return launch2<BN, true, QFX_EPI_BIAS>(P, s);
-      case QFX_EPI_DGELU: return launch2<BN, true, QFX_EPI_DGELU>(P, s);
-      case QFX_EPI_ADD: return launch2<BN, true, QFX_EPI_ADD>(P, s);
-      case QFX_EPI_ATTN_DO: return launch2<BN, true, QFX_EPI_ATTN_DO>(P, s);
-    }
-  }
-  set_error("qfx_gemm_bf16: unsupported (trans_b=%d, epilogue=%d)", trans_b, epi);
-  return -1;
 }
 
 template <int BN>
@@ -769,19 +418,14 @@ extern "C" int qfx_gemm_bf16(const qfx_gemm_problem* probs, int nprob, int N, in
                              int lora_group_n, int block_n, void* stream) {
   QFX_CHECK_ARG(nprob >= 1 && nprob <= QFX_MAX_PROBLEMS, "qfx_gemm_bf16: nprob=%d", nprob);
   QFX_CHECK_ARG(K > 0 && K % BK == 0, "qfx_gemm_bf16: K=%d must be a positive multiple of 64", K);
-  // block_n = 1000 + {128, 256}: CTA-pair (cta_group::2) kernel with 256-row tiles.  Auto (block_n = 0): the pair kernel whenever
-  // N is a multiple of 256 (1.37-1.56 PFLOP/s vs 1.17-1.32 for the single-CTA kernel on the block projections; QFX_GEMM_1CTA=1
-  // forces the single-CTA kernel for A/B comparisons).
-  static const bool force_1cta = getenv("QFX_GEMM_1CTA") != nullptr;
-  if (block_n == 0 && N % 256 == 0 && !force_1cta) block_n = 1256;
-  const bool two_cta = block_n >= 1000;
-  if (two_cta) block_n -= 1000;
+  // block_n = 1000 + bn asks for 256-row tiles computed by a CTA pair; the sm_90a library has one kernel with 128-row tiles and
+  // runs such a request as block_n = bn (the result is the same).
+  if (block_n >= 1000) block_n -= 1000;
   int bn = block_n;
   if (bn == 0 && epilogue == QFX_EPI_ATTN_DO) bn = N % 256 == 0 ? 256 : 128;  // a tile must hold whole heads
   if (bn == 0) bn = N % 256 == 0 ? 256 : N % 192 == 0 ? 192 : N % 128 == 0 ? 128 : 64;
   QFX_CHECK_ARG(epilogue != QFX_EPI_ATTN_DO || (trans_b && N % 128 == 0 && bn % 128 == 0), "qfx_gemm_bf16: ATTN_DO needs trans_b=1, N %% 128 == 0");
   QFX_CHECK_ARG((bn == 64 || bn == 128 || bn == 192 || bn == 256) && N % bn == 0, "qfx_gemm_bf16: N=%d block_n=%d", N, bn);
-  QFX_CHECK_ARG(!two_cta || bn == 128 || bn == 256, "qfx_gemm_bf16: the 2-CTA kernel takes block_n 128 or 256");
   QFX_CHECK_ARG(!(trans_b && lora_group_n), "qfx_gemm_bf16: lora_group_n only with trans_b=0");
   QFX_CHECK_ARG(lora_group_n == 0 || lora_group_n % bn == 0, "qfx_gemm_bf16: lora_group_n %% block_n != 0");
 
@@ -794,10 +438,11 @@ extern "C" int qfx_gemm_bf16(const qfx_gemm_problem* probs, int nprob, int N, in
   P.alpha = alpha;
   P.tiles_n = N / bn;
   {
+    // outputs larger than about the 50 MB L2 are streamed past it so that writing them does not evict the re-read A operand
     static const int force = getenv("QFX_GEMM_STREAM") ? atoi(getenv("QFX_GEMM_STREAM")) : -1;  // A/B switch
     double out_bytes = 0;
     for (int i = 0; i < nprob; ++i) out_bytes += 2.0 * probs[i].M * N * (epilogue == QFX_EPI_GELU ? 2 : 1);
-    P.stream_out = force >= 0 ? force : (out_bytes > 120e6);
+    P.stream_out = force >= 0 ? force : (out_bytes > 48e6);
   }
   int tiles_m_total = 0;
   for (int i = 0; i < nprob; ++i) {
@@ -808,7 +453,7 @@ extern "C" int qfx_gemm_bf16(const qfx_gemm_problem* probs, int nprob, int N, in
     int rc = make_2d(&d.tmA, s.A, (uint64_t)K, (uint64_t)s.M, s.lda, BK, BM);
     if (rc) return rc;
     if (!trans_b)
-      rc = make_2d(&d.tmB, s.B, (uint64_t)K, (uint64_t)N, s.ldb, BK, (uint32_t)(two_cta ? bn / 2 : bn));
+      rc = make_2d(&d.tmB, s.B, (uint64_t)K, (uint64_t)N, s.ldb, BK, (uint32_t)bn);
     else
       rc = make_2d(&d.tmB, s.B, (uint64_t)N, (uint64_t)K, s.ldb, 64, BK);
     if (rc) return rc;
@@ -820,7 +465,7 @@ extern "C" int qfx_gemm_bf16(const qfx_gemm_problem* probs, int nprob, int N, in
       rc = make_2d(&d.tmA2, s.A2, (uint64_t)(s.a2_col0 + 64 * s.kb2 * groups), (uint64_t)s.M, s.lda2, BK, BM);
       if (rc) return rc;
       if (!trans_b)
-        rc = make_2d(&d.tmB2, s.B2, (uint64_t)(64 * s.kb2), (uint64_t)N, s.ldb2, BK, (uint32_t)(two_cta ? bn / 2 : bn));
+        rc = make_2d(&d.tmB2, s.B2, (uint64_t)(64 * s.kb2), (uint64_t)N, s.ldb2, BK, (uint32_t)bn);
       else
         rc = make_2d(&d.tmB2, s.B2, (uint64_t)N, (uint64_t)(64 * s.kb2), s.ldb2, 64, BK);
       if (rc) return rc;
@@ -849,15 +494,14 @@ extern "C" int qfx_gemm_bf16(const qfx_gemm_problem* probs, int nprob, int N, in
                     "qfx_gemm_bf16: ATTN_DO row groups must share delta / attn_S / attn_H");
       P.delta = s.delta; P.attn_S = s.attn_S; P.attn_H = s.attn_H;
     }
-    int tm = two_cta ? (s.M + 255) / 256 : (s.M + BM - 1) / BM;
-    if (s.row_tiles) tm = two_cta ? s.n_row_tiles : 2 * s.n_row_tiles;
+    int tm = (s.M + BM - 1) / BM;
+    if (s.row_tiles) tm = 2 * s.n_row_tiles;
     tiles_m_total += tm;
     P.tiles_m_end[i] = tiles_m_total;
   }
   P.tiles_m_total = tiles_m_total;
   P.total_tiles = tiles_m_total * P.tiles_n;
   cudaStream_t st = (cudaStream_t)stream;
-  if (two_cta) return bn == 128 ? dispatch2<128>(P, trans_b, epilogue, st) : dispatch2<256>(P, trans_b, epilogue, st);
   switch (bn) {
     case 64: return dispatch<64>(P, trans_b, epilogue, st);
     case 128: return dispatch<128>(P, trans_b, epilogue, st);

@@ -9,7 +9,7 @@
 
 #include "../../include/qfx.h"
 #include "host_common.h"
-#include "sm100.cuh"
+#include "sm90.cuh"
 
 namespace qfx {
 

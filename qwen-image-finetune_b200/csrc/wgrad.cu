@@ -1,19 +1,19 @@
-// LoRA weight gradients on tcgen05:  G += A^T B  reduced over the token dimension M (split across CTAs).
+// LoRA weight gradients on wgmma:  G += A^T B  reduced over the token dimension M (split across CTAs).
 //   dB[out, r] = dY^T (s X A^T)        dA[r, in] = (s dY B)^T X         (autograd of peft's LoRA Linear,
 //   injected at /root/reference/src/qflux/trainer/base_trainer.py:929-941)
 // Both operands are row-major [M, cols] activations, i.e. the reduction dimension is the OUTER one — exactly the
-// MN-major UMMA operand layout — so TMA tiles of the tensors as they lie in HBM feed the tensor core directly:
-//   A tile [64 rows(m) x 128 cols] = 2 swizzle atoms   -> MMA "M" = 128 A-columns
+// MN-major wgmma operand layout — so TMA tiles of the tensors as they lie in HBM feed the tensor core directly:
+//   A tile [64 rows(m) x 128 cols] = 2 swizzle atoms   -> one M = 64 wgmma per consumer warpgroup and atom
 //   B tile [64 rows(m) x 64*NG cols] = NG atoms        -> MMA "N" = 64*NG (LoRA rank padded to 64 per group)
 // mode 0 (dA of a fused q|k|v site, or any single site): every A-column tile pairs with all NG groups of B.
 // mode 1 (dB of a fused site): A columns [g*Dg, (g+1)*Dg) pair with B group g only.
-// The [128 x 64*NG] fp32 accumulator lives in TMEM; the epilogue adds the first r columns of each group into the flat
+// The [128 x 64*NG] fp32 accumulator lives in the registers of two consumer warpgroups; the epilogue adds the first r columns of each group into the flat
 // fp32 LoRA-gradient buffer with red.global.add.f32 (a few thousand per CTA).
 #include <string.h>
 
 #include "../../include/qfx.h"
 #include "host_common.h"
-#include "sm100.cuh"
+#include "sm90.cuh"
 
 namespace qfx {
 
@@ -27,18 +27,21 @@ struct WgradParams {
 };
 
 template <int NG>
-__global__ void __launch_bounds__(192, 1) wgrad_kernel(const __grid_constant__ WgradParams P) {
+__device__ __forceinline__ void wgmma_wgrad(float* d, uint64_t a, uint64_t b, int scale_d) {
+  if constexpr (NG == 1) wgmma_ss_n64<1, 1>(d, a, b, scale_d);
+  else if constexpr (NG == 2) wgmma_ss_n128<1, 1>(d, a, b, scale_d);
+  else wgmma_ss_n192<1, 1>(d, a, b, scale_d);
+}
+
+template <int NG>
+__global__ void __launch_bounds__(384, 1) wgrad_kernel(const __grid_constant__ WgradParams P) {
   constexpr int A_BYTES = 2 * 8192, B_BYTES = NG * 8192, STAGE = A_BYTES + B_BYTES, STAGES = 4;
-  constexpr int TCOLS = NG == 1 ? 64 : NG == 2 ? 128 : 256;
   extern __shared__ uint8_t smem_raw[];
   const uint32_t smem_base = (smem_u32(smem_raw) + 1023u) & ~1023u;
   const uint32_t bar_base = smem_base + STAGES * STAGE;
   auto full_bar = [&](int s) { return bar_base + 8u * s; };
   auto empty_bar = [&](int s) { return bar_base + 8u * (STAGES + s); };
-  const uint32_t acc_bar = bar_base + 8u * (2 * STAGES);
-  const uint32_t tmem_slot = bar_base + 8u * (2 * STAGES + 1);
-  uint8_t* smem_gen = smem_raw + (smem_base - smem_u32(smem_raw));
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int wg = threadIdx.x >> 7;
 
   const int i0 = blockIdx.x * 128;                       // first A column of this tile
   const int m_begin = blockIdx.y * P.rows_per_split;
@@ -47,22 +50,17 @@ __global__ void __launch_bounds__(192, 1) wgrad_kernel(const __grid_constant__ W
   const int grp = P.mode == 1 ? i0 / P.Dg : 0;           // mode 1: the single B group this tile pairs with
   const int b_col0 = P.mode == 1 ? grp * 64 : 0;
 
-  if (warp == 1 && lane == 0) {
+  if (threadIdx.x == 0) {
     for (int s = 0; s < STAGES; ++s) {
       mbar_init(full_bar(s), 1);
-      mbar_init(empty_bar(s), 1);
+      mbar_init(empty_bar(s), 8);  // lane 0 of each consumer warp
     }
-    mbar_init(acc_bar, 1);
     fence_barrier_init();
   }
-  if (warp == 0) tmem_alloc(tmem_slot, TCOLS);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *reinterpret_cast<volatile uint32_t*>(smem_gen + (tmem_slot - smem_base));
 
-  if (warp == 0) {
-    if (lane == 0) {
+  if (wg == 0) {
+    if (threadIdx.x == 0) {
       tma_prefetch_desc(&P.tmA);
       tma_prefetch_desc(&P.tmB);
       for (int kb = 0; kb < nkb; ++kb) {
@@ -77,52 +75,47 @@ __global__ void __launch_bounds__(192, 1) wgrad_kernel(const __grid_constant__ W
         for (int g = 0; g < NG; ++g) tma_load_2d(b_dst + g * 8192, &P.tmB, full_bar(s), b_col0 + g * 64, m0);
       }
     }
-  } else if (warp == 1) {
-    if (lane == 0) {
-      constexpr uint32_t idesc = idesc_bf16(128, 64 * NG, 1, 1);
-      for (int kb = 0; kb < nkb; ++kb) {
-        const int s = kb % STAGES;
-        mbar_wait(full_bar(s), (kb / STAGES) & 1);
-        tc_fence_after();
-        const uint32_t a_addr = smem_base + s * STAGE, b_addr = a_addr + A_BYTES;
-#pragma unroll
-        for (int k = 0; k < 4; ++k)
-          umma_bf16(tmem_base, sdesc_sw128(a_addr + k * 2048, 8192, 1024), sdesc_sw128(b_addr + k * 2048, 8192, 1024), idesc,
-                    (kb | k) != 0);
-        umma_commit(empty_bar(s));
-      }
-      umma_commit(acc_bar);
-    }
   } else {
-    const int quad = warp & 3;
-    const int i = i0 + quad * 32 + lane;  // A column == accumulator row
-    mbar_wait(acc_bar, 0);
-    tc_fence_after();
-    const uint32_t t_row = tmem_base + ((uint32_t)(quad * 32) << 16);
-#pragma unroll 1
-    for (int g = 0; g < NG; ++g) {
-#pragma unroll 1
-      for (int c = 0; c < 64; c += 32) {
-        if (c >= P.r) break;
-        uint32_t v[32];
-        tmem_ld32(t_row + g * 64 + c, v);
-        tmem_ld_wait();
-        if (i < P.Na && nkb > 0) {
-          const int gg = P.mode == 1 ? grp : g;
-          const int64_t ii = P.mode == 1 ? (int64_t)(i - grp * P.Dg) : (int64_t)i;
-          float* dst = P.G[gg] + ii * P.gs_i;
+    // consumer cw: A columns i0 + 64 cw .. + 63 (one MN-major swizzle atom of the A tile) x all 64*NG B columns
+    const int cw = wg - 1;
+    const int t = threadIdx.x & 127, w = t >> 5, l = t & 31;
+    float acc[NG * 32];
 #pragma unroll
-          for (int e = 0; e < 32; ++e)
-            if (c + e < P.r) atomicAdd(dst + (int64_t)(c + e) * P.gs_j, __uint_as_float(v[e]));
+    for (int e = 0; e < NG * 32; ++e) acc[e] = 0.f;
+    reg_fence(acc, NG * 32);
+    for (int kb = 0; kb < nkb; ++kb) {
+      const int s = kb % STAGES;
+      mbar_wait(full_bar(s), (kb / STAGES) & 1);
+      const uint32_t a_addr = smem_base + s * STAGE + cw * 8192, b_addr = smem_base + s * STAGE + A_BYTES;
+      wgmma_fence();
+#pragma unroll
+      for (int k = 0; k < 4; ++k)
+        wgmma_wgrad<NG>(acc, sdesc_sw128(a_addr + k * 2048, 8192, 1024), sdesc_sw128(b_addr + k * 2048, 8192, 1024), 1);
+      wgmma_commit();
+      wgmma_wait<0>();
+      reg_fence(acc, NG * 32);
+      if (l == 0) mbar_arrive(empty_bar(s));
+    }
+    if (nkb > 0) {
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        const int i = i0 + cw * 64 + 16 * w + (l >> 2) + 8 * h;  // A column == accumulator row
+        if (i >= P.Na) continue;
+#pragma unroll
+        for (int jj = 0; jj < NG * 8; ++jj) {
+#pragma unroll
+          for (int e = 0; e < 2; ++e) {
+            const int col = 8 * jj + 2 * (l & 3) + e;
+            const int g = col >> 6, j = col & 63;
+            if (j < P.r) {
+              const int gg = P.mode == 1 ? grp : g;
+              const int64_t ii = P.mode == 1 ? (int64_t)(i - grp * P.Dg) : (int64_t)i;
+              atomicAdd(P.G[gg] + ii * P.gs_i + (int64_t)j * P.gs_j, acc[4 * jj + 2 * h + e]);
+            }
+          }
         }
       }
     }
-  }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 0) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, TCOLS);
   }
 }
 
@@ -134,7 +127,7 @@ static int launch_wgrad(const WgradParams& P, dim3 grid, cudaStream_t st) {
     QFX_CUDA(cudaFuncSetAttribute(wgrad_kernel<NG>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM));
     done = true;
   }
-  wgrad_kernel<NG><<<grid, 192, SMEM, st>>>(P);
+  wgrad_kernel<NG><<<grid, 384, SMEM, st>>>(P);
   QFX_CUDA(cudaGetLastError());
   return 0;
 }

@@ -1,4 +1,4 @@
-"""In-tree build of libqfx_b200.so:  nvcc -gencode arch=compute_100a,code=sm_100a  (cross-compiles without a GPU)."""
+"""In-tree build of libqfx_b200.so:  nvcc -gencode arch=compute_90a,code=sm_90a  (cross-compiles without a GPU)."""
 from __future__ import annotations
 
 import os
@@ -12,7 +12,7 @@ ROOT = os.path.dirname(os.path.dirname(HERE))
 LIB = os.path.join(HERE, "libqfx_b200.so")
 OBJ = os.path.join(CSRC, "_obj")
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
-FLAGS = ["-gencode", "arch=compute_100a,code=sm_100a", "-O3", "-std=c++17", "-lineinfo", "-Xcompiler", "-fPIC",
+FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-std=c++17", "-lineinfo", "-Xcompiler", "-fPIC",
          "--use_fast_math", "-I", os.path.join(ROOT, "include")]
 
 

@@ -67,7 +67,7 @@ class FluxB200(FusedMMDiTBase):
     def __init__(self, cfg: FluxB200Config, device="cuda", _host_only: bool = False):
         super().__init__()
         self._init_common(device, _host_only)
-        assert cfg.attention_head_dim == 128, "the sm_100a attention kernels are specialised for head_dim 128"
+        assert cfg.attention_head_dim == 128, "the sm_90a attention kernels are specialised for head_dim 128"
         self.config = cfg
         D = cfg.num_attention_heads * cfg.attention_head_dim
         self.D, self.H, self.J = D, cfg.num_attention_heads, cfg.joint_attention_dim

@@ -12,7 +12,7 @@ LIB_PATH = os.path.join(_HERE, "libqfx_b200.so")
 if not os.path.exists(LIB_PATH):
     raise ImportError(
         f"{LIB_PATH} is missing — build it with `python -c 'import __graft_entry__ as g; g.build()'` "
-        "(there is no CPU / eager fallback for the B200 hot path)")
+        "(there is no CPU / eager fallback for the CUDA hot path)")
 
 _lib = C.CDLL(LIB_PATH)
 _lib.qfx_last_error.restype = C.c_char_p
@@ -397,7 +397,7 @@ _wgrad_tc = _sig("qfx_lora_wgrad_tc", _vp, _i64, _i, _vp, _i64, _i, _i, _i, _i, 
 
 
 def lora_wgrad_tc(A, B, G_list, gs_i, gs_j, r, mode=0, Dg=0):
-    """tcgen05 LoRA weight gradient: G_g += A^T B_g over rows.  A [M, Na], B [M, 64*G] bf16; G_list: fp32 tensors (one per
+    """wgmma LoRA weight gradient: G_g += A^T B_g over rows.  A [M, Na], B [M, 64*G] bf16; G_list: fp32 tensors (one per
     group).  mode 0: all A columns pair with every group; mode 1: A columns [g*Dg, (g+1)*Dg) pair with group g only."""
     require_cuda(A, B, *G_list)
     n = len(G_list)

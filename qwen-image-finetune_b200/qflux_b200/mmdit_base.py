@@ -85,7 +85,7 @@ class FusedMMDiTBase(nn.Module):
     # -----------------------------------------------------------------------------------------------------------------
     def _init_common(self, device, host_only):
         if not host_only and not torch.cuda.is_available():
-            raise lib.QfxError(f"{type(self).__name__} needs a CUDA device (sm_100a); there is no CPU fallback")
+            raise lib.QfxError(f"{type(self).__name__} needs a CUDA device (sm_90a); there is no CPU fallback")
         self.dev = torch.device(device)
         self.sites = {}          # (l, grp, s) -> LoraSite   (l = -1: input embedders)
         self.mod_sites = {}      # kind -> dict(idx=[row indices], names=[...], A=[n, r, D], B=[n, C, r], ga, gb)  (AdaLN linears)
@@ -693,7 +693,7 @@ class FusedMMDiTBase(nn.Module):
         lib.lora_wgrad_tc(dY, Tb, gB, r, 1, r, mode=1 if site.n > 1 else 0, Dg=n_out_each if site.n > 1 else 0)
         if Xsaved.shape[1] % 128 == 0:
             lib.lora_wgrad_tc(Xsaved, U, gA, 1, Xsaved.shape[1], r, mode=0)
-        else:  # 64-channel latent embedder: too narrow for the tcgen05 tile, a [r, 64] result on the CUDA cores
+        else:  # 64-channel latent embedder: too narrow for the wgmma tile, a [r, 64] result on the CUDA cores
             for g in range(site.n):
                 lib.lora_wgrad(Xsaved, U[:, g * PAD:(g + 1) * PAD], gA[g], 1, Xsaved.shape[1], r)
         return U, site.A_pad, site.n

@@ -4,13 +4,13 @@ Mirrors the interface of the reference's `QwenImageTransformer2DModel`
 (/root/reference/src/qflux/models/transformer_qwenimage.py:497-672; called at
 /root/reference/src/qflux/trainer/qwen_image_edit_trainer.py:827-836): same forward kwargs, same state-dict key
 names (diffusers + PEFT `base_layer` / `lora_A.default` / `lora_B.default`), LoRA A/B exposed as nn.Parameters whose
-names contain "lora".  Every FLOP runs in libqfx_b200.so (hand-written sm_100a kernels); this file only sequences the
+names contain "lora".  Every FLOP runs in libqfx_b200.so (hand-written sm_90a kernels); this file only sequences the
 launches and owns the HBM layout (see mmdit_base.py / DESIGN.md §3):
 
   * frozen weights live in layer-stacked fused tensors (q|k|v concatenated per stream, both streams adjacent) so one
-    grouped tcgen05 GEMM serves the image and text stream of a block;
+    grouped wgmma GEMM serves the image and text stream of a block;
   * LoRA factors live zero-padded to 64 rows/cols so they enter the K loop of the base GEMM as one extra k-block;
-  * activations needed by the backward are kept in HBM (no recompute of GEMMs; 180 GB per GPU has room at B=4):
+  * activations needed by the backward are kept in HBM (no recompute of GEMMs; on an 80 GB H100 they are what limits the batch):
     block inputs, LayerNorm statistics, pre-norm q|k|v, attention output + logsumexp, mid residual, MLP pre-activation.
 
 No CPU path, no eager-PyTorch fallback: every op raises if the tensors are not on a CUDA device.
@@ -83,7 +83,7 @@ class QwenImageB200(FusedMMDiTBase):
         every compute entry point still raises on non-CUDA tensors."""
         super().__init__()
         self._init_common(device, _host_only)
-        assert cfg.attention_head_dim == 128, "the sm_100a attention kernels are specialised for head_dim 128"
+        assert cfg.attention_head_dim == 128, "the sm_90a attention kernels are specialised for head_dim 128"
         self.config = cfg
         # Multi-resolution batches with PADDED TEXT: "aligned" rotates a sample's image tokens where they sit ([T, T + L_b)), which makes
         # a padded batch equal the per-sample runs; "reference" reproduces transformer_qwen_custom.py:199-208, which lays the image table

@@ -12,8 +12,8 @@ parallel mode.  B200-first layout instead of FSDP's per-module flat parameters:
     starts, so NVLink traffic overlaps the ~6 ms of tensor-core work of a block;
   * on one node the gather is NOT a collective: the weights are frozen, so every rank exports its shard once through CUDA IPC
     (include/qfx.h qfx_peer_*) and a block is assembled by `world` copy-engine pulls over NVLink (cudaMemcpyAsync from the mapped
-    peer pointers, starting at the next rank so the NVSwitch ports are loaded evenly).  No SM is taken from the GEMMs — the NCCL
-    all-gather cost 14 % of the step at 2 GPUs (profiles/r02_bench_qwen_plus_sharded_2gpu_nccl_gather.json) — and no rank waits
+    peer pointers, starting at the next rank so the NVSwitch ports are loaded evenly).  No SM is taken from the GEMMs (an NCCL
+    all-gather runs kernels that would) and no rank waits
     for another.  `gather="nccl"` (or QFX_SHARD_GATHER=nccl, or ranks on different hosts) keeps the all_gather_into_tensor path;
   * kernels keep reading plain row-major [out, in] views — the views now point into the gather buffer of the block's slot.
 """

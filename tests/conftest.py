@@ -11,7 +11,7 @@ for p in (ROOT, PKG):
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a real B200 (run with -m gpu under gpurun)")
+    config.addinivalue_line("markers", "gpu: needs a real H100 (run with -m gpu)")
 
 
 def pytest_collection_modifyitems(config, items):

@@ -2,7 +2,7 @@
 
 Two uses:
   * `-m "not gpu"` tests monkey-patch it over `qflux_b200.lib` to exercise the host-side orchestration (launch order,
-    operand wiring, LoRA registry, gradient offsets) of the B200 model on CPU against the oracle;
+    operand wiring, LoRA registry, gradient offsets) of the fused model on CPU against the oracle;
   * `-m gpu` tests use the same functions as the "plain PyTorch fp32 reference of the same op" for each CUDA kernel.
 It is never imported by the product package.
 """

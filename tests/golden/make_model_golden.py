@@ -18,6 +18,9 @@ ROOT = os.path.dirname(os.path.dirname(os.path.dirname(os.path.abspath(__file__)
 sys.path.insert(0, ROOT)
 from oracle import mmdit_oracle as mo  # noqa: E402
 
+sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
+import ref_common as rc  # noqa: E402
+
 
 def _perturb(orc, seed):
     g = torch.Generator().manual_seed(seed)
@@ -28,7 +31,7 @@ def _perturb(orc, seed):
             elif p.ndim == 1:
                 p.copy_(1 + torch.randn(p.shape, generator=g) * 0.1)
         for p in orc.parameters():
-            p.copy_(p.bfloat16().float())  # bf16-representable weights: the B200 path stores bf16
+            p.copy_(p.bfloat16().float())  # bf16-representable weights: the fused path stores bf16
 
 
 def qwen_case(heads, hd, joint, axes, seed):
@@ -108,7 +111,7 @@ def main():
   for c in out.values():
       sd = c.pop("state_dict")
       c["weight_checksum"] = float(sum(v.double().abs().sum() for v in sd.values()))
-  torch.save(out, os.path.join(os.path.dirname(os.path.abspath(__file__)), "model_golden.pt"))
+  torch.save(rc._compact(out), os.path.join(os.path.dirname(os.path.abspath(__file__)), "model_golden.pt"))  # < 1 MB
   print({k: (float(v["loss"]), v["pred"].shape) for k, v in out.items()})
 
 

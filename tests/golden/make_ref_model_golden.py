@@ -1,4 +1,4 @@
-"""Generate tests/golden/ref_model_golden.pt by running the REFERENCE's OWN code (build container only; needs /root/reference):
+"""Generate tests/golden/ref_model_golden_*.pt (split below 1 MB per file) by running the REFERENCE's OWN code (build container only; needs /root/reference):
 
     python tests/golden/make_ref_model_golden.py
 
@@ -6,7 +6,7 @@ What runs is /root/reference/src/qflux itself — `QwenImageTransformer2DModel`,
 models, `BaseTrainer.add_lora_adapter`, `QwenImageEditTrainer._compute_loss` (+ `_get_sigmas`), `FluxKontextLoraTrainer._compute_loss`
 (shared and multi-resolution mode), `qflux.losses.*` — with `diffusers` / `peft` / `accelerate` replaced by the leaf restatements of
 tests/shims (tests/shims/README.md).  Stored per case: the embeddings dict handed to the trainer, the noise / u / t it drew, the
-model prediction, the loss and every LoRA gradient (fp32, CPU).  The GPU box never runs this; it reads the committed .pt file.
+model prediction, the loss and every LoRA gradient (fp32, CPU).  The GPU machine never runs this; it reads the committed .pt files.
 """
 import os
 import sys
@@ -152,8 +152,8 @@ def main():
         c = out[name]
         print(f"{name:28s} loss={float(c['loss']):.6f} pred={tuple(c['pred'].shape)} |pred|={float(c['pred'].abs().mean()):.4f} "
               f"n_lora={len(c['grads'])} |g|={float(sum(g.norm() ** 2 for g in c['grads'].values()) ** 0.5):.4e}")
-    torch.save(out, os.path.join(HERE, "ref_model_golden.pt"))
-    print("wrote", os.path.join(HERE, "ref_model_golden.pt"), os.path.getsize(os.path.join(HERE, "ref_model_golden.pt")) // 1024, "KiB")
+    for path in rc.save_split(out, HERE, "ref_model_golden"):
+        print("wrote", path, os.path.getsize(path) // 1024, "KiB")
 
 
 if __name__ == "__main__":

@@ -1,9 +1,11 @@
 """Shared by tests/golden/make_ref_model_golden.py (which imports the REFERENCE's own model / trainer code) and by the tests that check
 the oracle, the emulated host path and the CUDA path against the vectors it wrote.  Nothing here imports /root/reference.
 
-Weights are a pure function of (parameter name, shape, seed): the reference model, the oracle and the B200 model share the diffusers /
+Weights are a pure function of (parameter name, shape, seed): the reference model, the oracle and the fused model share the diffusers /
 PEFT state-dict key names, so filling each by name gives all three identical weights without shipping them."""
 import zlib
+
+import os
 
 import torch
 
@@ -65,7 +67,7 @@ def bf16_exact(t: torch.Tensor) -> torch.Tensor:
 
 @torch.no_grad()
 def det_fill_(model: torch.nn.Module, seed: int, w_std: float = 0.05, lora_b_std: float = 0.05) -> float:
-    """Fill every parameter from its NAME (bf16-representable values; the B200 path stores bf16).  Returns a checksum."""
+    """Fill every parameter from its NAME (bf16-representable values; the fused path stores bf16).  Returns a checksum."""
     tot = 0.0
     for name, p in sorted(model.named_parameters(), key=lambda kv: kv[0]):
         name = name.replace(".base_layer.", ".")  # PEFT wraps adapted Linears: the frozen weight keeps its diffusers name here
@@ -98,7 +100,7 @@ def rand_inputs(spec: dict) -> dict:
         L = shapes[0][1] * shapes[0][2]
         Lc = sum(f * h * w for f, h, w in shapes[1:])
         # u -> idx = (u * 1000).long() -> sigma = (1000 - idx) / 1000 in {0.5, 0.25, 0.75, 0.125}: bf16-exact, because the model rounds
-        # sigma to the working dtype before the 1000x sinusoid (transformer_qwenimage.py:624) and the B200 path works in bf16
+        # sigma to the working dtype before the 1000x sinusoid (transformer_qwenimage.py:624) and the fused path works in bf16
         x = dict(image_latents=rn(B, L, 64), control_latents=rn(B, Lc, 64), prompt_embeds=rn(B, T, J) * 3,
                  prompt_embeds_mask=torch.ones(B, T, dtype=torch.int64), img_shapes=[list(shapes)] * B,
                  u=torch.tensor([0.5, 0.75, 0.25, 0.875][:B]))
@@ -137,3 +139,53 @@ def rand_inputs(spec: dict) -> dict:
 def rel_l2(a: torch.Tensor, b: torch.Tensor) -> float:
     a, b = a.double(), b.double()
     return ((a - b).norm() / (b.norm() + 1e-30)).item()
+
+
+# ------------------------------------------------------------------------------------------------ golden files
+GOLDEN_PART_BYTES = 900_000  # every stored file stays below 1 MB
+
+
+def _compact(o):
+    """Deep copy with every tensor cloned: a saved view would drag its whole base storage into the file."""
+    if torch.is_tensor(o):
+        return o.clone()
+    if isinstance(o, dict):
+        return {k: _compact(v) for k, v in o.items()}
+    if isinstance(o, (list, tuple)):
+        return type(o)(_compact(v) for v in o)
+    return o
+
+
+def save_split(cases: dict, directory: str, stem: str) -> list:
+    """torch.save the per-case dict as stem_0.pt, stem_1.pt, ... (whole cases per file, each file < GOLDEN_PART_BYTES)."""
+    import io
+    parts, cur, cur_bytes = [], {}, 0
+    for name, c in cases.items():
+        c = _compact(c)
+        buf = io.BytesIO()
+        torch.save(c, buf)
+        n = len(buf.getvalue())
+        assert n < GOLDEN_PART_BYTES, f"golden case {name} alone is {n} bytes"
+        if cur and cur_bytes + n > GOLDEN_PART_BYTES:
+            parts.append(cur)
+            cur, cur_bytes = {}, 0
+        cur[name], cur_bytes = c, cur_bytes + n
+    if cur:
+        parts.append(cur)
+    for f in os.listdir(directory):
+        if f.startswith(stem + "_") and f.endswith(".pt"):
+            os.remove(os.path.join(directory, f))
+    paths = []
+    for i, part in enumerate(parts):
+        paths.append(os.path.join(directory, f"{stem}_{i}.pt"))
+        torch.save(part, paths[-1])
+    return paths
+
+
+def load_split(directory: str, stem: str) -> dict:
+    out = {}
+    names = sorted(f for f in os.listdir(directory) if f.startswith(stem + "_") and f.endswith(".pt"))
+    assert names, f"no {stem}_*.pt in {directory}"
+    for f in names:
+        out.update(torch.load(os.path.join(directory, f), weights_only=False))
+    return out

@@ -1,4 +1,4 @@
-"""The C-ABI library builds for sm_100a without a GPU, loads, and exports every symbol include/qfx.h declares."""
+"""The C-ABI library builds for sm_90a without a GPU, loads, and exports every symbol include/qfx.h declares."""
 import ctypes
 import os
 import re

@@ -26,7 +26,8 @@ GEMM = ["basic_nt_bn64", "basic_nn_bn64", "basic_nt_bn128", "basic_nn_bn128", "b
         "basic_nt_bn256", "basic_nn_bn256", "basic_nt_alpha_nobias", "basic_nt_big", "basic_nn_big", "lora_nt_bn128",
         "lora_nn_bn128", "lora_nt_bn256", "lora_nn_bn256", "lora_nt_groups3", "lora_nt_kb2", "lora_nn_kb3",
         "epilogues_bn128", "epilogues_bn256", "grouped_nt", "grouped_nn",
-        # CTA-pair kernel (cta_group::2), incl. the split-K tail wave (workspace + last-arriver epilogue)
+        # block_n = 1000 + bn (a request for 256-row CTA-pair tiles, served by the 128-row sm_90a kernel): the request path, plus the
+        # long-K shapes of the *_splitk cases (K = 4096-4608: 64-72 k-blocks per tile, many turns of the 4-6 stage TMA ring)
         "cta2_basic_nt_bn1256", "cta2_basic_nn_bn1256", "cta2_lora_nt_bn1256", "cta2_lora_nn_bn1256", "cta2_basic_nt_bn1128",
         "cta2_lora_nn_bn1128", "cta2_epilogues", "cta2_grouped_nt", "cta2_grouped_nn", "cta2_splitk_epilogues", "cta2_splitk_lora_nt",
         "cta2_splitk_lora_nn", "cta2_splitk_grouped_nn",

@@ -1,4 +1,4 @@
-"""Host-side logic of the B200 model (launch sequencing, operand wiring, LoRA registry, gradient offsets) on CPU:
+"""Host-side logic of the fused model (launch sequencing, operand wiring, LoRA registry, gradient offsets) on CPU:
 `qflux_b200.lib` is replaced by the plain-PyTorch emulation in tests/emu_lib.py and the result is compared with the oracle.
 (The CUDA kernels themselves are covered by the `-m gpu` tests.)"""
 import pytest
@@ -262,7 +262,7 @@ def test_qwen_multi_resolution_matches_per_sample_oracle(emu):
         total = total + ((p - (noise[b, :lt[b]].float() - x0[b, :lt[b]].float())) ** 2).mean(-1).sum()
     loss_o = total / (sum(lt) + 1e-12)
     loss_o.backward()
-    # ---- B200 (emulated kernels): one padded batch
+    # ---- fused model (emulated kernels): one padded batch
     step = QwenImageEditStep(m, "attention_mask")
     emb = dict(image_latents=x0, control_latents=ctrl, prompt_embeds=pe, prompt_embeds_mask=mask, img_shapes=shapes)
     loss_b = step.compute_loss(emb, noise=noise, u=u)
@@ -338,7 +338,7 @@ def test_flux_multi_resolution_matches_per_sample_oracle(emu):
         total = total + ((p - (noise[b, :lt[b]].float() - x0[b, :lt[b]].float())) ** 2).mean(-1).sum()
     loss_o = total / (sum(lt) + 1e-12)
     loss_o.backward()
-    # ---- B200 (emulated kernels): one padded batch
+    # ---- fused model (emulated kernels): one padded batch
     step = FluxKontextStep(m, "attention_mask")
     emb = dict(image_latents=x0, control_latents=ctrl, pooled_prompt_embeds=pooled, prompt_embeds=pe, text_ids=text_ids, img_shapes=shapes)
     loss_b = step.compute_loss(emb, noise=noise, t=t)

@@ -1,11 +1,11 @@
-"""Parity PIN: tests/golden/ref_model_golden.pt holds outputs of the REFERENCE'S OWN code (its model classes, its LoRA injection, its
+"""Parity PIN: tests/golden/ref_model_golden_*.pt hold outputs of the REFERENCE'S OWN code (its model classes, its LoRA injection, its
 trainers' `_compute_loss`, its losses — run through the leaf restatements of tests/shims; generator: tests/golden/make_ref_model_golden.py).
 
   * CPU: `oracle/mmdit_oracle.py` reproduces every case to fp32 round-off (pred / loss 1e-5, LoRA grads 1e-4) — this is what pins the
     oracle, and with it every "CUDA vs oracle" parity claim, to the reference;
-  * CPU: the B200 host path with emulated kernels reproduces the head_dim-128 cases at the bf16 tolerances;
+  * CPU: the fused host path with emulated kernels reproduces the head_dim-128 cases at the bf16 tolerances;
   * GPU (`-m gpu`): the CUDA path reproduces the head_dim-128 cases directly against the reference's vectors (no oracle in between).
-Tolerances (relative L2, reference convention tests/src/models/test_qwen_custom.py:550): bf16 B200 path vs fp32 reference: pred 2e-2
+Tolerances (relative L2, reference convention tests/src/models/test_qwen_custom.py:550): bf16 fused path vs fp32 reference: pred 2e-2
 (what the reference itself accepts for bf16, test_qwen_custom.py:635-636; measured 4e-3 .. 1.1e-2, the largest with LoRA on every Linear), |loss| 1e-2,
 LoRA gradients 2e-2 (3e-2 on the GPU where attention runs in bf16 tensor-core arithmetic)."""
 import os
@@ -18,7 +18,7 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 sys.path.insert(0, os.path.join(HERE, "golden"))
 import ref_common as rc  # noqa: E402
 
-G = torch.load(os.path.join(HERE, "golden", "ref_model_golden.pt"))
+G = rc.load_split(os.path.join(HERE, "golden"), "ref_model_golden")
 
 
 def _oracle(spec):
@@ -88,7 +88,7 @@ def test_oracle_matches_reference(name):
             assert (g - ref).norm() <= 1e-4 * ref.norm() + 1e-7, (n, rc.rel_l2(g, ref))
 
 
-# ------------------------------------------------------------------------------------------------------------------ B200 path
+# ------------------------------------------------------------------------------------------------------------------ fused path
 B200_CASES = ["qwen_hd128", "qwen_hd128_plus3", "qwen_hd128_alltargets", "qwen_hd128_editmask", "flux_hd128", "flux_hd128_yaml",
               "flux_custom_multires", "qwen_custom_multires"]
 
@@ -127,7 +127,7 @@ def _b200_step(name, device, host_only, tol_pred, tol_grad):
     from qflux_b200.train_step import FluxKontextStep, QwenImageEditStep
     spec, c = rc.CASES[name], G[name]
     m, chk = _b200_model(spec, device, host_only)
-    assert abs(chk - c["weight_checksum"]) <= 1e-9 * c["weight_checksum"], "B200 state-dict key set differs from the reference's"
+    assert abs(chk - c["weight_checksum"]) <= 1e-9 * c["weight_checksum"], "fused state-dict key set differs from the reference's"
     x, ex, kind = c["inputs"], c["extra"], spec["kind"]
     bf = lambda t: t.to(device).bfloat16()
     if kind == "qwen":

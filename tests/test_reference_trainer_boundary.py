@@ -1,6 +1,8 @@
-"""Row (b) of SURVEY.md §8 — the drop-in boundary — exercised with the REFERENCE'S OWN trainer code (build container only: needs
-/root/reference; `diffusers` / `peft` / `accelerate` come from tests/shims).  The fused model runs on CPU with emulated kernels
-(tests/emu_lib.py): what is under test is the interface, not the arithmetic.
+"""Row (b) of SURVEY.md §8 — the drop-in boundary — exercised with the REFERENCE'S OWN trainer code (tests that take the `ref` fixture
+need the reference checkout at /root/reference and skip without it; `diffusers` / `peft` / `accelerate` come from tests/shims).  What
+the reference computes as plain data — RoPE tables, sampling schedules, a cache directory it wrote — is stored in
+tests/golden/boundary_golden.pt (tests/golden/make_boundary_golden.py), so those comparisons run everywhere.  The fused model runs on
+CPU with emulated kernels (tests/emu_lib.py): what is under test is the interface, not the arithmetic.
 
 Driven reference code: `BaseTrainer.add_lora_adapter`, `.load_pretrain_lora_model`, `.save_lora`, `.clip_gradients`, `.forward_loss`,
 `QwenImageEditTrainer._compute_loss`, `utils.lora_utils.get_lora_layers / classify_lora_weight`, `QwenEmbedRope`,
@@ -13,7 +15,7 @@ import pytest
 import torch
 
 HERE = os.path.dirname(os.path.abspath(__file__))
-pytestmark = pytest.mark.skipif(not os.path.isdir("/root/reference/src/qflux"), reason="needs /root/reference (build container)")
+REF_SRC = "/root/reference/src"
 
 sys.path.insert(0, os.path.join(HERE, "golden"))
 sys.path.insert(0, os.path.join(HERE, "shims"))
@@ -21,12 +23,19 @@ sys.path.insert(0, os.path.join(HERE, "shims"))
 
 @pytest.fixture(scope="module")
 def ref():
+    if not os.path.isdir(os.path.join(REF_SRC, "qflux")):
+        pytest.skip("runs the reference's trainer code: needs the reference checkout at /root/reference")
     import stub_importer
     stub_importer.install()
-    if "/root/reference/src" not in sys.path:
-        sys.path.insert(0, "/root/reference/src")
+    if REF_SRC not in sys.path:
+        sys.path.insert(0, REF_SRC)
     import make_ref_model_golden as mg
     return mg
+
+
+@pytest.fixture(scope="module")
+def golden():
+    return torch.load(os.path.join(HERE, "golden", "boundary_golden.pt"), weights_only=False)
 
 
 @pytest.fixture()
@@ -74,14 +83,12 @@ def test_reference_add_lora_adapter_and_module_scan(ref, emu):
         m.to(torch.float32)                                  # ... re-typing the fused HBM layout is refused loudly
 
 
-def test_pos_embed_matches_reference_rope(ref):
+def test_pos_embed_matches_reference_rope(golden):
     """`dit.pos_embed([shapes], [T], device)` (qwen_image_edit_trainer.py:734) vs the reference's QwenEmbedRope (scale_rope=True)."""
-    from qflux.models.transformer_qwenimage import QwenEmbedRope
     m = _fused()
-    r = QwenEmbedRope(theta=10000, axes_dim=[16, 56, 56], scale_rope=True)
-    for shapes, T in (([(1, 4, 4), (1, 4, 4)], 7), ([(1, 4, 6), (1, 4, 6), (1, 2, 8)], 11)):
-        a_v, a_t = m.pos_embed([shapes], [T], device=torch.device("cpu"))
-        b_v, b_t = r([shapes], [T], device=torch.device("cpu"))
+    for c in golden["rope"]:
+        a_v, a_t = m.pos_embed([c["shapes"]], [c["T"]], device=torch.device("cpu"))
+        b_v, b_t = c["vid"], c["txt"]
         assert a_v.shape == b_v.shape and a_t.shape == b_t.shape
         assert (a_v - b_v).abs().max() < 2e-5 and (a_t - b_t).abs().max() < 2e-5
 
@@ -251,69 +258,41 @@ def test_patch_trainer_flux_shared_and_multires(ref, emu):
         assert set(g_r) <= set(g_b) and float((num / den).sqrt()) < 2e-2, case
 
 
-def test_sampler_schedule_matches_reference_prepare_predict_timesteps(ref):
+def test_sampler_schedule_matches_reference_prepare_predict_timesteps(golden):
     """§8 f2: `flow_match_sigmas` vs the reference's `BaseTrainer.prepare_predict_timesteps` (base_trainer.py:1009-1043 -> calculate_shift,
     retrieve_timesteps -> FlowMatchEulerDiscreteScheduler.set_timesteps(sigmas=, mu=)), for the Qwen-Image and the FLUX scheduler configs,
     and the Euler update vs `scheduler.step`."""
-    import contextlib
-    import io
-    from diffusers.schedulers.scheduling_flow_match_euler_discrete import FlowMatchEulerDiscreteScheduler
-    from qflux.trainer.base_trainer import BaseTrainer
-    from qflux.utils.sampling import calculate_shift as ref_shift
-    from qflux_b200.sampler import calculate_shift, flow_match_sigmas
-    qwen = dict(num_train_timesteps=1000, shift=1.0, use_dynamic_shifting=True, base_shift=0.5, max_shift=0.9, base_image_seq_len=256,
-                max_image_seq_len=8192, shift_terminal=0.02)
-    flux = dict(num_train_timesteps=1000, shift=3.0, use_dynamic_shifting=True, base_shift=0.5, max_shift=1.15, base_image_seq_len=256,
-                max_image_seq_len=4096)
-    for conf in (qwen, flux):
-        for steps, seq in ((20, 1024), (8, 4096), (50, 400)):
-            tr = types.SimpleNamespace(sampling_scheduler=FlowMatchEulerDiscreteScheduler(**conf), scheduler=None,
-                                       dit=torch.nn.Linear(1, 1))
-            with contextlib.redirect_stdout(io.StringIO()):  # the reference prints the shift arguments
-                ts, n = BaseTrainer.prepare_predict_timesteps(tr, steps, seq)
-                assert abs(calculate_shift(seq, conf["base_image_seq_len"], conf["max_image_seq_len"], conf["base_shift"], conf["max_shift"])
-                           - ref_shift(seq, conf["base_image_seq_len"], conf["max_image_seq_len"], conf["base_shift"], conf["max_shift"])) < 1e-12
-            sig = flow_match_sigmas(steps, seq, base_seq_len=conf["base_image_seq_len"], max_seq_len=conf["max_image_seq_len"],
-                                    base_shift=conf["base_shift"], max_shift=conf["max_shift"], shift_terminal=conf.get("shift_terminal"))
-            assert n == steps and sig.numel() == steps + 1 and sig[-1] == 0
-            assert torch.allclose(sig[:-1] * 1000, ts.cpu(), rtol=2e-6, atol=1e-4), (conf, steps, seq)
-            assert torch.allclose(sig, tr.sampling_scheduler.sigmas.cpu(), rtol=2e-6, atol=1e-7)
-            # one Euler step of the loop in sampler.py == scheduler.step (fp32 update, model dtype out)
-            x, v = torch.randn(2, 8, 64).bfloat16(), torch.randn(2, 8, 64).bfloat16()
-            tr.sampling_scheduler.set_begin_index(0)
-            want = tr.sampling_scheduler.step(v, ts[0], x, return_dict=False)[0]
-            from qflux_b200.sampler import _euler_step
-            got = _euler_step(x, v, sig, 0)
-            assert torch.equal(want, got)
+    from qflux_b200.sampler import _euler_step, calculate_shift, flow_match_sigmas
+    assert {c["config"] for c in golden["schedules"]} == {"qwen", "flux"} and len(golden["schedules"]) == 6
+    for c in golden["schedules"]:
+        conf, steps, seq, ts = c["conf"], c["steps"], c["seq"], c["timesteps"]
+        assert abs(calculate_shift(seq, conf["base_image_seq_len"], conf["max_image_seq_len"], conf["base_shift"], conf["max_shift"])
+                   - c["shift"]) < 1e-12
+        sig = flow_match_sigmas(steps, seq, base_seq_len=conf["base_image_seq_len"], max_seq_len=conf["max_image_seq_len"],
+                                base_shift=conf["base_shift"], max_shift=conf["max_shift"], shift_terminal=conf.get("shift_terminal"))
+        assert c["n"] == steps and sig.numel() == steps + 1 and sig[-1] == 0
+        assert torch.allclose(sig[:-1] * 1000, ts, rtol=2e-6, atol=1e-4), (c["config"], steps, seq)
+        assert torch.allclose(sig, c["sigmas"], rtol=2e-6, atol=1e-7)
+        # one Euler step of the loop in sampler.py == scheduler.step (fp32 update, model dtype out)
+        assert torch.equal(c["euler"], _euler_step(c["x"], c["v"], sig, 0))
 
 
-def test_loader_reads_a_cache_written_by_the_reference(ref, tmp_path):
-    """f3: the cache directory is produced by the reference's own `EmbeddingCacheManager.save_cache_embedding` (data/cache_manager.py:
-    46-93) and read back two ways — by the reference's `load_cache` and by `CachedEmbeddingLoader` — which must agree sample by sample
-    (values, fp16 storage, pixel `img_shapes` converted to latent-patch units, pad-to-max collate like `pad_to_max_shape`)."""
-    from qflux.data.cache_manager import EmbeddingCacheManager
-    from qflux.utils.tools import pad_to_max_shape
+def test_loader_reads_a_cache_written_by_the_reference(golden, tmp_path):
+    """f3: the cache directory was produced by the reference's own `EmbeddingCacheManager.save_cache_embedding` (data/cache_manager.py:
+    46-93); `CachedEmbeddingLoader` must read back what the reference's `load_cache` + `pad_to_max_shape` (utils/tools.py:399-425) read
+    from it, sample by sample (values, fp16 storage, pixel `img_shapes` converted to latent-patch units, pad-to-max collate)."""
     from qflux_b200.cache_loader import CachedEmbeddingLoader
-    mgr = EmbeddingCacheManager(str(tmp_path))
-    g = torch.Generator().manual_seed(5)
-    sizes, hashes = [(512, 512), (320, 640), (640, 384)], []
-    for i, (H, W) in enumerate(sizes):
-        L, T = (H // 16) * (W // 16), 6 + 5 * i
-        data = dict(image_latents=torch.randn(L, 64, generator=g), control_latents=torch.randn(L, 64, generator=g),
-                    prompt_embeds=torch.randn(T, 48, generator=g))
-        fh = dict(main_hash=f"m{i:03d}", image_hash=f"i{i:03d}", control_hash=f"c{i:03d}", prompt_hash=f"p{i:03d}")
-        mgr.save_cache_embedding(data, dict(image_latents="image_hash", control_latents="control_hash", prompt_embeds="prompt_hash"), fh,
-                                 img_shapes=[[3, H, W], [3, H, W]])
-        hashes.append(fh)
-    assert EmbeddingCacheManager.exist(str(tmp_path))
+    c = golden["cache"]
+    for rel, data in c["files"].items():
+        p = tmp_path / rel
+        p.parent.mkdir(parents=True, exist_ok=True)
+        p.write_bytes(data)
     ours = list(CachedEmbeddingLoader(str(tmp_path), batch_size=3, device="cpu", shuffle=False, drop_last=False))
     assert len(ours) == 1
     b = ours[0]
-    theirs = [mgr.load_cache({"file_hashes": fh}) for fh in hashes]  # the reference's reader, one sample at a time
-    for key in ("image_latents", "control_latents", "prompt_embeds"):
-        want = pad_to_max_shape([t[key] for t in theirs])  # the reference's collate (utils/tools.py:399-425)
+    for key, want in c["want"].items():
         assert b[key].dtype == torch.float16 and torch.equal(b[key], want), key
-    assert b["img_shapes"] == [[(1, H // 16, W // 16)] * 2 for H, W in sizes]
+    assert b["img_shapes"] == [[(1, H // 16, W // 16)] * 2 for H, W in c["sizes"]]
     assert b["prompt_embeds_mask"].sum(1).tolist() == [6, 11, 16]
     # ... and the same batch again from the packed shards written off that cache
     from qflux_b200.cache_loader import pack_cache

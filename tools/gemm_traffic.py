@@ -1,6 +1,6 @@
 """Time the step's big grouped GEMMs stand-alone (CUDA events, L2 flushed) — run it under `ncu --metrics dram__bytes_read.sum,
 dram__bytes_write.sum,gpu__time_duration.sum` to get the DRAM traffic per launch (tools/ncu_traffic.py turns the csv into
-profiles/r02_ncu_traffic.json).  Shapes: Qwen-Image-Edit B=4 (8192 image + 1408 text rows)."""
+a DRAM-traffic capture).  Shapes: Qwen-Image-Edit B=4 (8192 image + 1408 text rows)."""
 import os
 import sys
 

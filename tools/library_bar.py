@@ -1,4 +1,4 @@
-"""GPU library bar (BASELINE.md §2): what the reference would actually run on one B200 — the eager-PyTorch restatement of its step
+"""GPU library bar (BASELINE.md §2): what the reference would actually run on one H100 — the eager-PyTorch restatement of its step
 (cuBLASLt bf16 GEMMs + F.scaled_dot_product_attention, autograd backward, torch AdamW on the LoRA parameters) — and the library
 attention kernels (cuDNN / flash SDPA, forward and backward) at the benchmark shape, timed beside our own kernels.
 
@@ -154,7 +154,7 @@ def step_ckpt():
 
 
 def step_nockpt():
-    """Without checkpointing the eager activations of 60 blocks at B=4 do not fit 180 GB: measure the deepest model that fits and
+    """Without checkpointing the eager activations of 60 blocks at B=4 do not fit one GPU: measure the deepest model that fits and
     scale linearly in depth (the embed / head share is < 1 %)."""
     for layers in (60, 40, 28, 20, 12):
         try:

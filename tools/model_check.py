@@ -1,7 +1,7 @@
 """GPU parity of the fused Qwen-Image training step against the pure-torch oracle (run under gpurun).
 
 The oracle runs on the same GPU in fp32 (reference numerics) and in bf16 (the reference's eager working dtype); the
-B200 path is compared with both using the reference's own metric, relative L2 (tests/src/models/test_qwen_custom.py:550).
+fused path is compared with both using the reference's own metric, relative L2 (tests/src/models/test_qwen_custom.py:550).
 """
 import os
 import sys
@@ -29,7 +29,7 @@ def build_pair(H, L, J, r, targets, seed=0, b_std=0.05, w_std=0.05):
     if r:
         mo.add_lora_adapter(orc, r=r, alpha=r, target_modules=targets, seed=seed, b_std=b_std)
     orc = orc.cuda()
-    # quantise every parameter to bf16 once so that fp32-oracle, bf16-oracle and the B200 model share identical weights
+    # quantise every parameter to bf16 once so that fp32-oracle, bf16-oracle and the fused model share identical weights
     with torch.no_grad():
         for p in orc.parameters():
             p.copy_(p.bfloat16().float())
@@ -62,7 +62,7 @@ def step_parity(H=2, L=2, J=128, B=2, hw=4, T=24, r=4, targets=("to_q", "to_k", 
     loss_o, pred_o = mo.qwen_compute_loss(orc, **xf)
     loss_o.backward()
     g_o = {n: (p.grad.clone() if p.grad is not None else torch.zeros_like(p)) for n, p in orc.named_parameters() if p.requires_grad}
-    # ---- B200
+    # ---- fused model
     step = QwenImageEditStep(m)
     emb = {k: x[k] for k in ("image_latents", "control_latents", "prompt_embeds", "img_shapes")}
     loss_b = step.compute_loss(emb, noise=x["noise"], u=x["u"])
@@ -125,7 +125,7 @@ def bench_point_6blk():
     image tokens, LoRA r=16 — fused step vs the fp32 and the bf16 oracle (cross-block strides, the B=4 batch indexing of the modulation
     vectors, the grouped text+image launches at their real sizes).  Also the ragged-mask variant [352, 300, 352, 257]: the stock Qwen
     forward hands `attention_mask=None` to SDPA and uses only max(txt_seq_lens) for the RoPE table (transformer_qwenimage.py:226-232,
-    332-339), so its result must EQUAL the all-ones-mask result — checked on the oracle and on the B200 module path."""
+    332-339), so its result must EQUAL the all-ones-mask result — checked on the oracle and on the fused module path."""
     from oracle import mmdit_oracle as mo
     t0 = time.time()
     r = step_parity(H=24, L=6, J=3584, B=4, hw=32, T=352, r=16, bf16_oracle=True)
@@ -149,7 +149,7 @@ def bench_point_6blk():
                                      return_dict=False)[0].float()
     r["ragged_mask_oracle_diff"] = float((outs["orc_ragged"] - outs["orc_ones"]).abs().max())
     # (the split-K tail of the GEMMs adds partial sums with red.global in arrival order: two launches differ in the last bf16 bit here and
-    # there, so the B200 comparison is a relative L2 against that run-to-run floor, not bit equality)
+    # there, so the fused comparison is a relative L2 against that run-to-run floor, not bit equality)
     r["ragged_mask_b200_diff"] = rel_l2(outs["b200_ragged"], outs["b200_ones"])
     r["ragged_b200_vs_bf16oracle"] = rel_l2(outs["b200_ragged"], outs["orc_ragged"])
     r["secs"] = round(time.time() - t0, 1)
@@ -157,7 +157,7 @@ def bench_point_6blk():
 
 
 def train_trajectory(steps=5, H=4, L=4, J=256, B=4, hw=8, T=40, r=8):
-    """`steps` optimizer steps: fused step + FusedLoraAdamW (clip 1.0) on the B200 path vs the fp32 oracle + clip_grad_norm_ +
+    """`steps` optimizer steps: fused step + FusedLoraAdamW (clip 1.0) on the fused path vs the fp32 oracle + clip_grad_norm_ +
     torch.optim.AdamW with the same noise / timestep draws — loss trajectory and final LoRA parameters."""
     from oracle import mmdit_oracle as mo
     from qflux_b200.optim import FusedLoraAdamW

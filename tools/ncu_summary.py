@@ -1,6 +1,6 @@
-"""Turn one `ncu --set full` capture (.ncu-rep, one kernel launch) into the markdown summary committed under profiles/.
+"""Turn one `ncu --set full` capture (.ncu-rep, one kernel launch) into a markdown summary.
 
-usage: python tools/ncu_summary.py gpurun_out/prof_x.ncu-rep "title" > profiles/r01_ncu_full_x.md
+usage: python tools/ncu_summary.py prof_x.ncu-rep "title" > summary.md
 """
 import csv
 import io

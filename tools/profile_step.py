@@ -1,4 +1,4 @@
-"""Run a few fused training steps at full width but reduced depth — the target of `ncu` captures (profiles/).
+"""Run a few fused training steps at full width but reduced depth — a target for profiler captures.
 Kernel SHARES per block are depth-independent; absolute step numbers from this script are NOT bench values."""
 import argparse
 import os
