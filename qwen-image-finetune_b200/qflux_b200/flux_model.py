@@ -18,7 +18,7 @@ from dataclasses import dataclass
 import torch
 
 from . import lib
-from .mmdit_base import BF, DEFAULT_TARGETS, PAD, FusedMMDiTBase, ModelFn  # noqa: F401
+from .mmdit_base import BF, DEFAULT_TARGETS, PAD, FusedMMDiTBase  # noqa: F401
 from .rope import flux_rope_table
 
 
@@ -50,19 +50,21 @@ FLUX_KONTEXT_YAML_TARGETS = (
     r"|.*(?<!single_)transformer_blocks\.[0-9]+\.ff_context\.net\.0\.proj|.*(?<!single_)transformer_blocks\.[0-9]+\.ff_context\.net\.2"
     r"|.*(?<!single_)transformer_blocks\.[0-9]+\.attn\.(to_add_out|add_k_proj|add_q_proj|add_v_proj))")
 
-_DOUBLE_LINEARS = {
-    "attn.to_q": ("qkv", 0, 0), "attn.to_k": ("qkv", 0, 1), "attn.to_v": ("qkv", 0, 2),
-    "attn.add_q_proj": ("qkv", 1, 0), "attn.add_k_proj": ("qkv", 1, 1), "attn.add_v_proj": ("qkv", 1, 2),
-    "attn.to_out.0": ("out", 0, 0), "attn.to_add_out": ("out", 1, 0),
-    "ff.net.0.proj": ("up", 0, 0), "ff_context.net.0.proj": ("up", 1, 0),
-    "ff.net.2": ("down", 0, 0), "ff_context.net.2": ("down", 1, 0),
-}
 _SINGLE_LINEARS = {"attn.to_q": ("s_qkv", 0), "attn.to_k": ("s_qkv", 1), "attn.to_v": ("s_qkv", 2), "proj_mlp": ("s_mlp", 0),
                    "proj_out": ("s_out", 0)}
 
 
 class FluxB200(FusedMMDiTBase):
     round_mid = False  # torch.nn.RMSNorm (transformer_flux.py:342-343): one rounding after the weight multiply
+    _DOUBLE_LINEARS = {
+        "attn.to_q": ("qkv", 0, 0), "attn.to_k": ("qkv", 0, 1), "attn.to_v": ("qkv", 0, 2),
+        "attn.add_q_proj": ("qkv", 1, 0), "attn.add_k_proj": ("qkv", 1, 1), "attn.add_v_proj": ("qkv", 1, 2),
+        "attn.to_out.0": ("out", 0, 0), "attn.to_add_out": ("out", 1, 0),
+        "ff.net.0.proj": ("up", 0, 0), "ff_context.net.0.proj": ("up", 1, 0),
+        "ff.net.2": ("down", 0, 0), "ff_context.net.2": ("down", 1, 0),
+    }
+    _ADALN = ("norm1.linear", "norm1_context.linear")
+    _PER_SINGLE = ("s_mod_w", "s_mod_b", "s_qkv_w", "s_qkv_b", "s_mlp_w", "s_mlp_b", "s_out_w", "s_out_b", "s_qknorm_w")
 
     def __init__(self, cfg: FluxB200Config, device="cuda", _host_only: bool = False):
         super().__init__()
@@ -115,19 +117,8 @@ class FluxB200(FusedMMDiTBase):
             out[p + "linear_2.weight"], out[p + "linear_2.bias"] = w[pre + "2_w"], w[pre + "2_b"]
         out["norm_out.linear.weight"], out["norm_out.linear.bias"] = w["norm_out_w"], w["norm_out_b"]
         out["proj_out.weight"], out["proj_out.bias"] = w["proj_out_w"], w["proj_out_b"]
-        sharded = self._sharded is not None  # sharded block weights are not addressable as full tensors
-        for l in range(0 if sharded else self.L):
-            b = f"transformer_blocks.{l}."
-            for s, nm in ((0, "norm1.linear"), (1, "norm1_context.linear")):
-                out[b + nm + ".weight"], out[b + nm + ".bias"] = w["mod_w"][l, s], w["mod_b"][l, s]
-            for i, nm in enumerate(("attn.norm_q", "attn.norm_k", "attn.norm_added_q", "attn.norm_added_k")):
-                out[b + nm + ".weight"] = w["qknorm_w"][l, i]
-            for nm, (grp, s, slot) in _DOUBLE_LINEARS.items():
-                W, Bv = w[grp + "_w"][l, s], w[grp + "_b"][l, s]
-                if grp == "qkv":
-                    W, Bv = W[slot * D:(slot + 1) * D], Bv[slot * D:(slot + 1) * D]
-                out[b + nm + ".weight"], out[b + nm + ".bias"] = W, Bv
-        for l in range(0 if sharded else self.Ls):
+        self._double_weight_views(out)
+        for l in range(self.Ls if self._sharded is None else 0):
             b = f"single_transformer_blocks.{l}."
             out[b + "norm.linear.weight"], out[b + "norm.linear.bias"] = w["s_mod_w"][l], w["s_mod_b"][l]
             out[b + "attn.norm_q.weight"], out[b + "attn.norm_k.weight"] = w["s_qknorm_w"][l, 0], w["s_qknorm_w"][l, 1]
@@ -138,64 +129,10 @@ class FluxB200(FusedMMDiTBase):
                 out[b + nm + ".weight"], out[b + nm + ".bias"] = W, Bv
         return out
 
-    _PER_LAYER = ("mod_w", "mod_b", "qkv_w", "qkv_b", "out_w", "out_b", "up_w", "up_b", "down_w", "down_b", "qknorm_w")
-    _PER_SINGLE = ("s_mod_w", "s_mod_b", "s_qkv_w", "s_qkv_b", "s_mlp_w", "s_mlp_b", "s_out_w", "s_out_b", "s_qknorm_w")
-
-    def shard_frozen_weights(self, group=None, gather="auto"):
-        """The reference's FSDP branch (base_trainer.py:333-382) for FLUX: 1/world of every double and every single block's frozen
-        weights per rank, a block assembled right before it runs (sharding.py; one two-slot ring per block kind).  LoRA factors
-        and the embedders / head stay replicated.  Call after the weights are loaded."""
-        from .sharding import ShardedBlocks
-        if self._sharded is not None:
-            return self
-        self._sharded = ShardedBlocks({k: self.w[k] for k in self._PER_LAYER}, self.L, group, gather=gather)
-        for k in self._PER_LAYER:
-            self.w[k] = self._sharded.rings[k]
-        self._sharded_s = None
-        if self.Ls:
-            self._sharded_s = ShardedBlocks({k: self.w[k] for k in self._PER_SINGLE}, self.Ls, group, gather=gather)
-            for k in self._PER_SINGLE:
-                self.w[k] = self._sharded_s.rings[k]
-        if torch.cuda.is_available():
-            torch.cuda.empty_cache()
-        return self
-
-    def _ring(self, blk):
-        """(ring, local index) of global block `blk` (double blocks first, then single blocks)."""
-        return (self._sharded, blk) if blk < self.L else (self._sharded_s, blk - self.L)
-
-    def _acquire(self, ws, blk, nxt):
-        """Sharded weights: make block `blk` resident, start fetching `nxt`, and produce blk's base modulation vectors."""
-        ring, l = self._ring(blk)
-        ring.acquire(l)
-        if 0 <= nxt < self.L + self.Ls:
-            r2, l2 = self._ring(nxt)
-            r2.prefetch(l2)
-
-    def _release(self, blk):
-        ring, l = self._ring(blk)
-        ring.release(l)
-
-    def _block_mods(self, ws, blk):
-        D, w = self.D, self.w
-        if blk < self.L:
-            lib.gemv_act(ws["temb"], w["mod_w"][blk].view(2 * 6 * D, D), w["mod_b"][blk].view(-1),
-                         ws["mods"][:, blk * 12 * D:(blk + 1) * 12 * D], act=1)
-            self._mod_lora_fwd(ws, ws["temb"], ("dbl", (2 * blk, 2 * blk + 1)))
-        else:
-            l = blk - self.L
-            lib.gemv_act(ws["temb"], w["s_mod_w"][l], w["s_mod_b"][l], ws["smods"][:, l * 3 * D:(l + 1) * 3 * D], act=1)
-            self._mod_lora_fwd(ws, ws["temb"], ("sgl", (l,)))
-
     def _linear_table(self) -> dict:
         D = self.D
-        dims = {"qkv": (D, D, 3), "out": (D, D, 1), "up": (D, 4 * D, 1), "down": (4 * D, D, 1),
-                "s_qkv": (D, D, 3), "s_mlp": (D, 4 * D, 1), "s_out": (5 * D, D, 1)}
-        t = {}
-        for l in range(self.L):
-            for nm, (grp, s, slot) in _DOUBLE_LINEARS.items():
-                d_in, d_out, n = dims[grp]
-                t[f"transformer_blocks.{l}.{nm}"] = ((l, grp), (s,), slot, d_in, d_out, n)
+        dims = {"s_qkv": (D, D, 3), "s_mlp": (D, 4 * D, 1), "s_out": (5 * D, D, 1)}
+        t = super()._linear_table()
         for l in range(self.Ls):
             for nm, (grp, slot) in _SINGLE_LINEARS.items():
                 d_in, d_out, n = dims[grp]
@@ -203,10 +140,7 @@ class FluxB200(FusedMMDiTBase):
         return t
 
     def _mod_table(self) -> dict:
-        t = {}
-        for l in range(self.L):
-            t[f"transformer_blocks.{l}.norm1.linear"] = ("dbl", 2 * l, 6)
-            t[f"transformer_blocks.{l}.norm1_context.linear"] = ("dbl", 2 * l + 1, 6)
+        t = super()._mod_table()
         for l in range(self.Ls):
             t[f"single_transformer_blocks.{l}.norm.linear"] = ("sgl", l, 3)
         return t
@@ -222,28 +156,13 @@ class FluxB200(FusedMMDiTBase):
             e = lambda *s, dt=BF: torch.empty(*s, device=self.dev, dtype=dt)
             for k in ("sin", "gsin"):
                 ws[k] = e(B, 256)
-            for k in ("e1", "temb", "gemb", "pemb", "tmp"):
+            for k in ("e1", "temb", "gemb", "pemb"):
                 ws[k] = e(B, D)
             ws["mods"] = e(B, self.L * 2 * 6 * D)
             ws["smods"] = e(B, max(self.Ls, 1) * 3 * D)
             ws["fmod"] = e(B, 2 * D)
-            if train:
-                ws["dqkv_s"] = ws["dqkv"]
             return ws
         return self._get_workspace((B, T, Limg, train), build)
-
-    def _mods(self, ws, l):
-        D = self.D
-
-        def f(j):
-            return tuple(ws["mods"][:, ((l * 2 + s) * 6 + j) * D: ((l * 2 + s) * 6 + j + 1) * D] for s in (0, 1))
-        return f
-
-    def _smod(self, ws, l, j):
-        """j-th chunk (shift, scale, gate) of single block l — the same [B, D] vector for both row groups."""
-        D = self.D
-        v = ws["smods"][:, (l * 3 + j) * D: (l * 3 + j + 1) * D]
-        return (v, v)
 
     # ------------------------------------------------------------------------------------------------ single block
     def _single_fwd(self, ws, l, Xin, Xout, save):
@@ -339,8 +258,7 @@ class FluxB200(FusedMMDiTBase):
             lib.add_bf16(ws["temb"], ws["gemb"], ws["temb"])
         self._mlp2(pooled_projections.to(BF).contiguous(), "p", ws["pemb"], ws["e1"])
         lib.add_bf16(ws["temb"], ws["pemb"], ws["temb"])
-        sh = self._sharded
-        if sh is None:  # all modulation linears of a kind in one launch; sharded weights produce them block by block
+        if self._sharded is None:  # all modulation linears of a kind in one launch; sharded weights produce them block by block
             lib.gemv_act(ws["temb"], w["mod_w"].view(L * 2 * 6 * D, D), w["mod_b"].view(-1), ws["mods"], act=1)
             if Ls:
                 lib.gemv_act(ws["temb"], w["s_mod_w"].view(Ls * 3 * D, D), w["s_mod_b"].view(-1), ws["smods"], act=1)
@@ -349,78 +267,17 @@ class FluxB200(FusedMMDiTBase):
         # --- embedders
         self._embed_fwd(ws, "x_in", 0, hidden_states.to(BF).reshape(B * Limg, self.C_in), X0[Mt:])
         self._embed_fwd(ws, "ctx_in", 1, encoder_hidden_states.to(BF).reshape(Mt, self.J), X0[:Mt])
-        # --- blocks
-        nb = L + Ls
-        xi = lambda i: ws["X"][i] if train else ws["X"][i & 1]
-        for blk in range(nb):
-            if sh is not None:
-                self._acquire(ws, blk, blk + 1)
-                self._block_mods(ws, blk)
-            if blk < L:
-                self._double_fwd(ws, blk, xi(blk), xi(blk + 1), ws["dbl"][blk if train else 0], self._mods(ws, blk))
-            else:
-                self._single_fwd(ws, blk - L, xi(blk), xi(blk + 1), ws["sgl"][(blk - L) if train else 0])
-            if sh is not None:
-                self._release(blk)
-        Xl = xi(nb)
-        ws["Xlast"] = Xl
-        lib.ln_modulate_fwd(Xl[Mt:], ws["hn"], ws["fmod"][:, D:], ws["fmod"][:, :D], Limg, ws["fstats"][0], ws["fstats"][1])
-        lib.gemm([lib.gemm_problem(ws["hn"], w["proj_out_w"], ws["pred"], bias=w["proj_out_b"])], self.C_out, D)
-        return ws["pred"].view(B, Limg, self.C_out)
-
-    # ------------------------------------------------------------------------------------------------ backward
-    def _last_gate(self, ws, blk):
-        """gate multiplying the residual branch that ENDS block `blk` (global index over double then single blocks)."""
-        return self._mods(ws, blk)(5) if blk < self.L else self._smod(ws, blk - self.L, 2)
-
-    def _backward_impl(self, dpred):
-        ws = self._ws
-        assert ws is not None and self._ws_key[3], "backward needs a training-mode forward first"
-        Limg, Mt = ws["Limg"], ws["Mt"]
-        D, L, Ls, w = self.D, self.L, self.Ls, self.w
-        nb = L + Ls
-        self._mod_grad_buffers(ws)
-        lib.gemm([lib.gemm_problem(dpred, w["proj_out_w"], ws["dhn"])], D, self.C_out, trans_b=True)
-        dX = ws["dX"][nb & 1]
-        dX[:Mt].zero_()
-        ws["dY"][:Mt].zero_()
-        lib.ln_modulate_bwd(ws["dhn"], ws["Xlast"][Mt:], ws["fstats"][0], ws["fstats"][1], ws["fmod"][:, :D], Limg, dX[Mt:],
-                            gate=self._last_gate(ws, nb - 1)[0], dx_gated=ws["dY"][Mt:])
-        for blk in range(nb - 1, -1, -1):
-            dXn = ws["dX"][blk & 1]
-            prev = self._last_gate(ws, blk - 1) if blk > 0 else None
-            if self._sharded is not None:
-                self._acquire(ws, blk, blk - 1)
-            if blk >= L:
-                self._single_bwd(ws, blk - L, ws["X"][blk], dX, dXn, ws["sgl"][blk - L], prev)
-            else:
-                self._double_bwd(ws, blk, ws["X"][blk], dX, dXn, ws["dbl"][blk], self._mods(ws, blk), prev)
-            if self._sharded is not None:
-                self._release(blk)
-            dX = dXn
-        self._mod_lora_bwd(ws)
-        self._embed_bwd(ws, "x_in", 0, dX)
-        self._embed_bwd(ws, "ctx_in", 1, dX)
+        return self._blocks_and_head_fwd(ws, train)
 
     # ------------------------------------------------------------------------------------------------ public API
     def forward(self, hidden_states, encoder_hidden_states=None, pooled_projections=None, timestep=None, img_ids=None,
                 txt_ids=None, guidance=None, joint_attention_kwargs=None, return_dict=False, attention_mask=None):
-        if torch.is_inference_mode_enabled():  # see QwenImageB200.forward: nothing of the model's state may become an inference tensor
-            with torch.inference_mode(False), torch.no_grad():
-                return self.forward(hidden_states, encoder_hidden_states, pooled_projections, timestep, img_ids, txt_ids, guidance,
-                                    joint_attention_kwargs, return_dict, attention_mask)
-        kv_len = None
-        if attention_mask is not None:  # [B, T + L] validity mask of a pad-to-max batch (prefix-valid per sample, tools.py:319-396)
-            kv_len = attention_mask.to(self.dev).sum(dim=1).to(torch.int32)
-            if img_ids.ndim == 2:
-                img_ids = img_ids[None].expand(hidden_states.shape[0], -1, -1)
-        args = (hidden_states, encoder_hidden_states, pooled_projections, timestep, img_ids, txt_ids, guidance, kv_len)
-        if torch.is_grad_enabled() and self._lora_params:
-            out = ModelFn.apply(self, args, *self._lora_params.values())
-        else:
-            out = self._infer(args).clone()
-        if kv_len is not None:  # padded image rows come back as exact zeros (transformer_flux_custom.py:724-735)
-            T = encoder_hidden_states.shape[1]
-            valid = torch.arange(out.shape[1], device=out.device)[None, :] < (kv_len[:, None] - T)
-            out = out * valid[..., None].to(out.dtype)
-        return (out,)
+        """Padded image rows of a pad-to-max batch (`attention_mask`) come back as exact zeros (transformer_flux_custom.py:724-735)."""
+        def make_args():
+            kv_len, ids = None, img_ids
+            if attention_mask is not None:  # [B, T + L] validity mask of a pad-to-max batch (prefix-valid per sample, tools.py:319-396)
+                kv_len = attention_mask.to(self.dev).sum(dim=1).to(torch.int32)
+                if ids.ndim == 2:
+                    ids = ids[None].expand(hidden_states.shape[0], -1, -1)
+            return (hidden_states, encoder_hidden_states, pooled_projections, timestep, ids, txt_ids, guidance, kv_len)
+        return self._forward_tail(make_args)

@@ -1,5 +1,6 @@
-"""Shared host-side machinery of the fused B200 MMDiT models (Qwen-Image, FLUX): HBM layout, LoRA registry, the
-double-stream block forward/backward launch sequences and the autograd bridge.  All arithmetic is in libqfx_b200.so.
+"""Shared host-side machinery of the fused B200 MMDiT models (Qwen-Image, FLUX): HBM layout, LoRA registry, sharded frozen
+weights, the double-stream block forward/backward launch sequences, the block stack with its output head, the CUDA-graph cache
+and the autograd bridge.  All arithmetic is in libqfx_b200.so.
 
 Layout conventions (DESIGN.md §3):
   * tokens are stream-major: rows [0, B*T) text (stream index 1), rows [B*T, B*T + B*L) image (stream index 0);
@@ -13,6 +14,7 @@ from __future__ import annotations
 import math
 import os
 import re
+import warnings
 
 import torch
 import torch.nn as nn
@@ -60,21 +62,54 @@ class FusedMMDiTBase(nn.Module):
     # subclasses fill these -------------------------------------------------------------------------------------------
     round_mid = True  # diffusers RMSNorm (Qwen) rounds before the weight multiply; torch.nn.RMSNorm (FLUX) does not
     keep_qkv = True   # keep normalised/rotated Q,K,V and the LN1 output of double blocks for the backward (HBM for time)
+    Ls = 0            # single-stream blocks (FLUX), run after the L double-stream blocks
+    _DOUBLE_LINEARS: dict = {}  # diffusers sub-module name of a double-block Linear -> (group, stream, slot); stream 0 = image, 1 = text
+    _ADALN = ("", "")           # sub-module names of a double block's (image, text) AdaLN modulation Linears
+    _PER_LAYER = ("mod_w", "mod_b", "qkv_w", "qkv_b", "out_w", "out_b", "up_w", "up_b", "down_w", "down_b", "qknorm_w")
+    _PER_SINGLE = ()
+    _sharded_s = None           # sharding.ShardedBlocks of the single blocks once shard_frozen_weights() has run
 
     def _weight_views(self) -> dict:
         raise NotImplementedError
 
+    def _double_weight_views(self, out: dict) -> dict:
+        """Adds the state-dict entries of every double block to `out` (sharded block weights are not addressable as full tensors)."""
+        w, D = self.w, self.D
+        for l in range(self.L if self._sharded is None else 0):
+            b = f"transformer_blocks.{l}."
+            for s, nm in enumerate(self._ADALN):
+                out[b + nm + ".weight"], out[b + nm + ".bias"] = w["mod_w"][l, s], w["mod_b"][l, s]
+            for i, nm in enumerate(("attn.norm_q", "attn.norm_k", "attn.norm_added_q", "attn.norm_added_k")):
+                out[b + nm + ".weight"] = w["qknorm_w"][l, i]
+            for nm, (grp, s, slot) in self._DOUBLE_LINEARS.items():
+                W, Bv = w[grp + "_w"][l, s], w[grp + "_b"][l, s]
+                if grp == "qkv":
+                    W, Bv = W[slot * D:(slot + 1) * D], Bv[slot * D:(slot + 1) * D]
+                out[b + nm + ".weight"], out[b + nm + ".bias"] = W, Bv
+        return out
+
     def _linear_table(self) -> dict:
         """full module name -> (site_key=(l, grp), streams tuple, slot, d_in, d_out, n_slots)"""
-        raise NotImplementedError
+        D = self.D
+        dims = {"qkv": (D, D, 3), "out": (D, D, 1), "up": (D, 4 * D, 1), "down": (4 * D, D, 1)}
+        t = {}
+        for l in range(self.L):
+            for nm, (grp, s, slot) in self._DOUBLE_LINEARS.items():
+                d_in, d_out, n = dims[grp]
+                t[f"transformer_blocks.{l}.{nm}"] = ((l, grp), (s,), slot, d_in, d_out, n)
+        return t
 
     def _mod_table(self) -> dict:
         """full name of an AdaLN modulation Linear -> (kind, index, n_chunks): kind "dbl" indexes rows of ws["mods"] viewed
         [B, L*2, 6D] (index = 2*l + stream), kind "sgl" rows of ws["smods"] viewed [B, Ls, 3D]."""
-        return {}
+        t = {}
+        for l in range(self.L):
+            for s, nm in enumerate(self._ADALN):
+                t[f"transformer_blocks.{l}.{nm}"] = ("dbl", 2 * l + s, 6)
+        return t
 
     def _embed_table(self) -> dict:
-        """full name of an input embedder Linear -> (weight key prefix in self.w, stream, d_in)."""
+        """full name of an input embedder Linear -> (weight key prefix in self.w, stream, d_in), image embedder first."""
         return {}
 
     def _wb(self, l, grp, s):
@@ -99,7 +134,7 @@ class FusedMMDiTBase(nn.Module):
         self.gradient_checkpointing = False  # accepted for interface compatibility; HBM holds the activations
         self._sharded = None     # sharding.ShardedBlocks once shard_frozen_weights() has run
         self._bands_cache = {}   # (valid image rows per sample, Limg) -> lib.RowBands (ragged GEMM row bands)
-        self._infer_graphs, self.use_cuda_graph_inference = {}, True  # captured no-grad forwards, by input signature (see _infer)
+        self._infer_graphs, self.use_cuda_graph_inference = GraphCache(8, "the inference forward"), True  # see _infer
         self._fwd_gen = 0        # bumped by every forward: autograd nodes of an older forward refuse to run (their activations are gone)
 
     @property
@@ -110,9 +145,53 @@ class FusedMMDiTBase(nn.Module):
     def dtype(self):
         return BF
 
-    def shard_frozen_weights(self, group=None):
-        """FSDP-style sharding of the frozen block weights (sharding.py); implemented for the Qwen-Image model (BASELINE config 4)."""
-        raise NotImplementedError(f"{type(self).__name__}: sharded frozen weights are implemented for QwenImageB200 only")
+    def shard_frozen_weights(self, group=None, gather="auto"):
+        """BASELINE config 4 (the reference's FSDP branch, base_trainer.py:333-382): keep 1/world of every double and every single
+        block's frozen weights on this rank; a block's full weights are assembled in one of two ring buffers right before it runs —
+        by copy-engine pulls from the peers' shards on one node, by an NCCL all-gather otherwise (sharding.py; one two-slot ring
+        per block kind).  Call after the weights are loaded.  LoRA factors, embedders and the output head stay replicated;
+        `state_dict()` then only carries the replicated tensors and the LoRA parameters."""
+        from .sharding import ShardedBlocks
+        if self._sharded is not None:
+            return self
+        self._sharded = ShardedBlocks({k: self.w[k] for k in self._PER_LAYER}, self.L, group, gather=gather)
+        for k in self._PER_LAYER:
+            self.w[k] = self._sharded.rings[k]
+        if self.Ls:
+            self._sharded_s = ShardedBlocks({k: self.w[k] for k in self._PER_SINGLE}, self.Ls, group, gather=gather)
+            for k in self._PER_SINGLE:
+                self.w[k] = self._sharded_s.rings[k]
+        if torch.cuda.is_available():
+            torch.cuda.empty_cache()
+        return self
+
+    def _ring(self, blk):
+        """(ring, local index) of global block `blk` (double blocks first, then single blocks)."""
+        return (self._sharded, blk) if blk < self.L else (self._sharded_s, blk - self.L)
+
+    def _acquire(self, blk, nxt):
+        """Sharded weights: make block `blk` resident and start fetching block `nxt` (if there is one)."""
+        ring, l = self._ring(blk)
+        ring.acquire(l)
+        if 0 <= nxt < self.L + self.Ls:
+            r2, l2 = self._ring(nxt)
+            r2.prefetch(l2)
+
+    def _release(self, blk):
+        ring, l = self._ring(blk)
+        ring.release(l)
+
+    def _block_mods(self, ws, blk):
+        """Sharded weights: the base modulation vectors of block `blk` (plus their LoRA), from its now resident weights."""
+        D, w = self.D, self.w
+        if blk < self.L:
+            lib.gemv_act(ws["temb"], w["mod_w"][blk].view(2 * 6 * D, D), w["mod_b"][blk].view(-1),
+                         ws["mods"][:, blk * 12 * D:(blk + 1) * 12 * D], act=1)
+            self._mod_lora_fwd(ws, ws["temb"], ("dbl", (2 * blk, 2 * blk + 1)))
+        else:
+            l = blk - self.L
+            lib.gemv_act(ws["temb"], w["s_mod_w"][l], w["s_mod_b"][l], ws["smods"][:, l * 3 * D:(l + 1) * 3 * D], act=1)
+            self._mod_lora_fwd(ws, ws["temb"], ("sgl", (l,)))
 
     def enable_gradient_checkpointing(self, *args, **kwargs):
         self.gradient_checkpointing = True
@@ -297,7 +376,8 @@ class FusedMMDiTBase(nn.Module):
         self._gnorm_sq = torch.zeros(1, device=self.dev, dtype=torch.float32)
         self._gscratch = torch.zeros(5 * self.D * PAD, device=self.dev, dtype=torch.float32)
         self._ws = self._ws_key = None  # per-block saved tensors depend on which sites exist
-        self._train_ws, self._infer_ws, self._infer_graphs = None, {}, {}
+        self._train_ws, self._infer_ws = None, {}
+        self._infer_graphs.clear()
         return self
 
     def _register_lora(self, full: str, pA: nn.Parameter, pB: nn.Parameter):
@@ -542,46 +622,28 @@ class FusedMMDiTBase(nn.Module):
     # A no-grad forward of 60 blocks is ~650 launches issued through ctypes: 40-65 ms of host time against 25 ms (B=1) to 95 ms (B=4) of
     # device time, and the validation sampler calls it 40 times per image (20 Euler steps x true CFG).  Like the training step, the second
     # forward of a given input signature is captured into a CUDA graph and later ones replay it (inputs copied into static buffers).
-    MAX_INFER_GRAPHS = 8
-
     def _infer(self, args):
         """`_forward_impl(*args, train=False)` -> prediction [B, Limg, C_out] (a view of workspace memory: callers clone it)."""
-        cuda = self.dev.type == "cuda" and torch.cuda.is_available()
-        if not cuda or not self.use_cuda_graph_inference or self._sharded is not None:
-            return self._forward_impl(*args, train=False)
-        key = _graph_sig(args)
-        ent = self._infer_graphs.get(key)
-        if ent is None:
-            if len(self._infer_graphs) >= self.MAX_INFER_GRAPHS:  # a caller that changes shapes every call stays eager
-                return self._forward_impl(*args, train=False)
-            self._infer_graphs[key] = "warm"
-            return self._forward_impl(*args, train=False)
-        if ent != "warm" and ent["ws"] is not self._ws and not self._activate_ws(ent["ws"], ent["ws_key"]):
-            ent = "warm"  # the workspace this graph was recorded on has been dropped: record again
-        if ent == "warm":
-            static = _graph_clone(args)
-            torch.cuda.synchronize()
-            g = torch.cuda.CUDAGraph()
-            n0 = lib.LAUNCHES
-            try:
-                with torch.cuda.graph(g):
-                    out = self._forward_impl(*static, train=False)
-            except Exception as e:
-                import warnings
-                warnings.warn(f"qflux_b200: CUDA-graph capture of the inference forward failed ({type(e).__name__}: {e}); running eagerly")
-                torch.cuda.synchronize()
-                self.use_cuda_graph_inference = False
-                lib.LAUNCHES = n0
-                return self._forward_impl(*args, train=False)
-            ent = dict(graph=g, static=static, out=out, launches=lib.LAUNCHES - n0, ws=self._ws, ws_key=self._ws_key,
-                       keep=tuple(self._ws.get(k) for k in ("rope", "kv_len", "txt_len", "bands")))
-            lib.LAUNCHES = n0
-            self._infer_graphs[key] = ent
-        _graph_copy(ent["static"], args)
-        ent["graph"].replay()
-        lib.LAUNCHES += ent["launches"]
-        self._fwd_gen += 1
-        return ent["out"]
+        return self._infer_graphs.run(self, lambda *a: self._forward_impl(*a, train=False), args, enabled=self.use_cuda_graph_inference)
+
+    def _forward_tail(self, make_args):
+        """The public `forward` once the family has turned its kwargs into `_forward_impl` arguments (`make_args()`): the fused
+        autograd bridge when grad is enabled and an adapter is attached, the (graphed) no-grad forward otherwise."""
+        if torch.is_inference_mode_enabled():
+            # the reference's validation loop runs under torch.inference_mode() (qwen_image_edit_trainer.py:1219): workspaces and cached
+            # tables allocated there would be inference tensors, which later no_grad / training calls may not update in place
+            with torch.inference_mode(False), torch.no_grad():
+                return self._forward_tail(make_args)
+        args = make_args()
+        if torch.is_grad_enabled() and self._lora_params:
+            out = ModelFn.apply(self, args, *self._lora_params.values())
+        else:
+            out = self._infer(args).clone()
+        kv = self._ws.get("kv_len")
+        if kv is not None:  # padded image rows of a multi-resolution batch are returned as exact zeros (test_qwen_custom.py:672-692)
+            valid = torch.arange(out.shape[1], device=out.device)[None, :] < (kv[:, None] - self._ws["T"])
+            out = out * valid[..., None].to(out.dtype)
+        return (out,)
 
     def _site(self, l, grp, s):
         return self.sites.get((l, grp, s))
@@ -844,6 +906,77 @@ class FusedMMDiTBase(nn.Module):
         lib.ln_modulate_bwd_pair(ws["dxm"], Xin, st[0], st[1], (mods(1)[1], T, pg[1]), (mods(1)[0], Limg, pg[0]), Mt, dXn, dres=dX,
                                  dx_gated=ws["dY"] if prev_gate else None)
 
+    # ------------------------------------------------------------------------------------------------ block stack and output head
+    def _mods(self, ws, l):
+        """j -> (image view, text view) of the j-th D-wide modulation chunk of double block l (shift1,scale1,gate1,shift2,scale2,gate2)."""
+        D = self.D
+
+        def f(j):
+            return tuple(ws["mods"][:, ((l * 2 + s) * 6 + j) * D: ((l * 2 + s) * 6 + j + 1) * D] for s in (0, 1))
+        return f
+
+    def _smod(self, ws, l, j):
+        """j-th chunk (shift, scale, gate) of single block l — the same [B, D] vector for both row groups."""
+        D = self.D
+        v = ws["smods"][:, (l * 3 + j) * D: (l * 3 + j + 1) * D]
+        return (v, v)
+
+    def _last_gate(self, ws, blk):
+        """gate multiplying the residual branch that ENDS block `blk` (global index over double then single blocks)."""
+        return self._mods(ws, blk)(5) if blk < self.L else self._smod(ws, blk - self.L, 2)
+
+    def _blocks_and_head_fwd(self, ws, train):
+        """Every block (double blocks, then single blocks) from the embedded tokens in ws["X"][0], then the output head on the image
+        rows: AdaLayerNormContinuous (scale, shift) + proj_out.  Returns the prediction [B, Limg, C_out] (workspace memory)."""
+        D, L, Mt, w, sh = self.D, self.L, ws["Mt"], self.w, self._sharded
+        nb = L + self.Ls
+        xi = lambda i: ws["X"][i] if train else ws["X"][i & 1]
+        for blk in range(nb):
+            if sh is not None:  # block blk's weights arrive by all-gather (block blk+1's gather starts now, on the side stream)
+                self._acquire(blk, blk + 1)
+                self._block_mods(ws, blk)
+            if blk < L:
+                self._double_fwd(ws, blk, xi(blk), xi(blk + 1), ws["dbl"][blk if train else 0], self._mods(ws, blk))
+            else:
+                self._single_fwd(ws, blk - L, xi(blk), xi(blk + 1), ws["sgl"][(blk - L) if train else 0])
+            if sh is not None:
+                self._release(blk)
+        Xl = ws["Xlast"] = xi(nb)
+        lib.ln_modulate_fwd(Xl[Mt:], ws["hn"], ws["fmod"][:, D:], ws["fmod"][:, :D], ws["Limg"], ws["fstats"][0], ws["fstats"][1])
+        lib.gemm([lib.gemm_problem(ws["hn"], w["proj_out_w"], ws["pred"], bias=w["proj_out_b"])], self.C_out, D)
+        return ws["pred"].view(ws["B"], ws["Limg"], self.C_out)
+
+    def _backward_impl(self, dpred):
+        """dpred: [B*Limg, C_out] bf16 gradient of the loss wrt the prediction; accumulates LoRA grads into self.G32."""
+        ws = self._ws
+        assert ws is not None and self._ws_key[3], "backward needs a training-mode forward first"
+        Limg, Mt = ws["Limg"], ws["Mt"]
+        D, L, w = self.D, self.L, self.w
+        nb = L + self.Ls
+        self._mod_grad_buffers(ws)
+        # --- head: proj_out dgrad -> final AdaLN backward.  Text rows of the last block output receive no gradient.
+        lib.gemm([lib.gemm_problem(dpred, w["proj_out_w"], ws["dhn"])], D, self.C_out, trans_b=True)
+        dX = ws["dX"][nb & 1]
+        dX[:Mt].zero_()
+        ws["dY"][:Mt].zero_()
+        lib.ln_modulate_bwd(ws["dhn"], ws["Xlast"][Mt:], ws["fstats"][0], ws["fstats"][1], ws["fmod"][:, :D], Limg, dX[Mt:],
+                            gate=self._last_gate(ws, nb - 1)[0], dx_gated=ws["dY"][Mt:])
+        for blk in range(nb - 1, -1, -1):
+            dXn = ws["dX"][blk & 1]
+            prev = self._last_gate(ws, blk - 1) if blk > 0 else None
+            if self._sharded is not None:
+                self._acquire(blk, blk - 1)
+            if blk < L:
+                self._double_bwd(ws, blk, ws["X"][blk], dX, dXn, ws["dbl"][blk], self._mods(ws, blk), prev)
+            else:
+                self._single_bwd(ws, blk - L, ws["X"][blk], dX, dXn, ws["sgl"][blk - L], prev)
+            if self._sharded is not None:
+                self._release(blk)
+            dX = dXn
+        self._mod_lora_bwd(ws)
+        for key, s, _ in self._embed_table().values():
+            self._embed_bwd(ws, key, s, dX)
+
     # ------------------------------------------------------------------------------------------------ workspace pieces
     def _alloc_common(self, ws, B, T, Limg, train, n_double, n_single=0):
         D, H = self.D, self.H
@@ -925,6 +1058,67 @@ class FusedMMDiTBase(nn.Module):
         if held:
             self._ws, self._ws_key = ws, key
         return held
+
+
+class GraphCache:
+    """CUDA graphs of a shape-static launch sequence `fn(*args)` of a model (the fused training step, the no-grad forward), one per
+    input signature, the least recently used dropped beyond `capacity` (every captured graph owns a private memory pool).
+
+    The first call of a signature runs eagerly (it allocates the workspace, RoPE tables and split-K scratch and sets kernel
+    attributes), the second captures `fn` on static copies of the inputs (kernel arguments, TMA descriptors included, are baked in)
+    and every later call copies its inputs into those buffers and replays.  Sharded frozen weights (side-stream all-gathers) and
+    non-CUDA models run eagerly; so does a cache whose capture failed once (with a warning: never silently wrong)."""
+
+    def __init__(self, capacity: int, what: str):
+        self.capacity, self.what = capacity, what
+        self.entries = {}  # key -> "warm" (seen once) | captured graph; most recently used last
+        self.failed = False
+
+    def captured(self) -> int:
+        return sum(isinstance(e, dict) for e in self.entries.values())
+
+    def clear(self):
+        self.entries.clear()
+
+    def run(self, model, fn, args, tag=None, enabled=True):
+        """fn(*args) through the graph of key (input signature, tag)."""
+        if not enabled or self.failed or model._sharded is not None or model.dev.type != "cuda" or not torch.cuda.is_available():
+            return fn(*args)
+        key = (_graph_sig(args), tag)
+        ent = self.entries.pop(key, None)
+        if ent is None:
+            while len(self.entries) >= self.capacity:
+                self.entries.pop(next(iter(self.entries)))
+            self.entries[key] = "warm"
+            return fn(*args)
+        self.entries[key] = ent
+        if ent != "warm" and ent["ws"] is not model._ws and not model._activate_ws(ent["ws"], ent["ws_key"]):
+            ent = "warm"  # the model dropped the workspace this graph was recorded on (another shape ran in between): record again
+        if ent == "warm":
+            static = _graph_clone(args)
+            torch.cuda.synchronize()
+            g = torch.cuda.CUDAGraph()
+            n0 = lib.LAUNCHES
+            try:
+                with torch.cuda.graph(g):
+                    out = fn(*static)
+            except Exception as e:
+                warnings.warn(f"qflux_b200: CUDA-graph capture of {self.what} failed ({type(e).__name__}: {e}); running eagerly")
+                torch.cuda.synchronize()
+                self.failed = True
+                lib.LAUNCHES = n0
+                return fn(*args)
+            # `keep`: per-shape tables the captured kernels point at (RoPE, key lengths, ragged row bands) live in bounded caches of the
+            # model — the graph must keep them alive after they are evicted there
+            ent = dict(graph=g, static=static, out=out, launches=lib.LAUNCHES - n0, ws=model._ws, ws_key=model._ws_key,
+                       keep=tuple(model._ws.get(k) for k in ("rope", "kv_len", "txt_len", "bands")))
+            lib.LAUNCHES = n0  # capture launches nothing
+            self.entries[key] = ent
+        _graph_copy(ent["static"], args)
+        ent["graph"].replay()
+        lib.LAUNCHES += ent["launches"]
+        model._fwd_gen += 1  # a replay is a forward that bypasses _forward_impl: autograd nodes of older forwards must refuse to run
+        return ent["out"]
 
 
 def _graph_sig(a):

@@ -22,7 +22,7 @@ from dataclasses import dataclass
 import torch
 
 from . import lib
-from .mmdit_base import BF, DEFAULT_TARGETS, PAD, FusedMMDiTBase, ModelFn  # noqa: F401
+from .mmdit_base import BF, DEFAULT_TARGETS, PAD, FusedMMDiTBase  # noqa: F401
 from .rope import qwen_rope_table
 
 
@@ -40,16 +40,6 @@ class QwenB200Config:
 
     def __getitem__(self, k):
         return getattr(self, k)
-
-
-# (diffusers sub-module name) -> (group, stream, slot).  stream 0 = image, 1 = text.
-_BLOCK_LINEARS = {
-    "attn.to_q": ("qkv", 0, 0), "attn.to_k": ("qkv", 0, 1), "attn.to_v": ("qkv", 0, 2),
-    "attn.add_q_proj": ("qkv", 1, 0), "attn.add_k_proj": ("qkv", 1, 1), "attn.add_v_proj": ("qkv", 1, 2),
-    "attn.to_out.0": ("out", 0, 0), "attn.to_add_out": ("out", 1, 0),
-    "img_mlp.net.0.proj": ("up", 0, 0), "txt_mlp.net.0.proj": ("up", 1, 0),
-    "img_mlp.net.2": ("down", 0, 0), "txt_mlp.net.2": ("down", 1, 0),
-}
 
 
 class _QwenPosEmbed:
@@ -77,6 +67,14 @@ class _QwenPosEmbed:
 
 class QwenImageB200(FusedMMDiTBase):
     round_mid = True
+    _DOUBLE_LINEARS = {
+        "attn.to_q": ("qkv", 0, 0), "attn.to_k": ("qkv", 0, 1), "attn.to_v": ("qkv", 0, 2),
+        "attn.add_q_proj": ("qkv", 1, 0), "attn.add_k_proj": ("qkv", 1, 1), "attn.add_v_proj": ("qkv", 1, 2),
+        "attn.to_out.0": ("out", 0, 0), "attn.to_add_out": ("out", 1, 0),
+        "img_mlp.net.0.proj": ("up", 0, 0), "txt_mlp.net.0.proj": ("up", 1, 0),
+        "img_mlp.net.2": ("down", 0, 0), "txt_mlp.net.2": ("down", 1, 0),
+    }
+    _ADALN = ("img_mod.1", "txt_mod.1")
 
     def __init__(self, cfg: QwenB200Config, device="cuda", _host_only: bool = False):
         """`_host_only=True` (tests of the naming / LoRA-registry logic) allocates on `device` without requiring CUDA;
@@ -112,7 +110,7 @@ class QwenImageB200(FusedMMDiTBase):
 
     # ------------------------------------------------------------------------------------------------ names
     def _weight_views(self) -> dict:
-        w, D, out = self.w, self.D, {}
+        w, out = self.w, {}
         out["img_in.weight"], out["img_in.bias"] = w["img_in_w"], w["img_in_b"]
         out["txt_norm.weight"] = w["txt_norm_w"]
         out["txt_in.weight"], out["txt_in.bias"] = w["txt_in_w"], w["txt_in_b"]
@@ -121,59 +119,12 @@ class QwenImageB200(FusedMMDiTBase):
         out[p + "linear_2.weight"], out[p + "linear_2.bias"] = w["t2_w"], w["t2_b"]
         out["norm_out.linear.weight"], out["norm_out.linear.bias"] = w["norm_out_w"], w["norm_out_b"]
         out["proj_out.weight"], out["proj_out.bias"] = w["proj_out_w"], w["proj_out_b"]
-        for l in range(self.L if self._sharded is None else 0):  # sharded block weights are not addressable as full tensors
-            b = f"transformer_blocks.{l}."
-            for s, nm in ((0, "img_mod.1"), (1, "txt_mod.1")):
-                out[b + nm + ".weight"], out[b + nm + ".bias"] = w["mod_w"][l, s], w["mod_b"][l, s]
-            for i, nm in enumerate(("attn.norm_q", "attn.norm_k", "attn.norm_added_q", "attn.norm_added_k")):
-                out[b + nm + ".weight"] = w["qknorm_w"][l, i]
-            for nm, (grp, s, slot) in _BLOCK_LINEARS.items():
-                W, Bv = w[grp + "_w"][l, s], w[grp + "_b"][l, s]
-                if grp == "qkv":
-                    W, Bv = W[slot * D:(slot + 1) * D], Bv[slot * D:(slot + 1) * D]
-                out[b + nm + ".weight"], out[b + nm + ".bias"] = W, Bv
-        return out
-
-    _PER_LAYER = ("mod_w", "mod_b", "qkv_w", "qkv_b", "out_w", "out_b", "up_w", "up_b", "down_w", "down_b", "qknorm_w")
-
-    def shard_frozen_weights(self, group=None, gather="auto"):
-        """BASELINE config 4 ("FSDP"): keep 1/world of every block's frozen weights on this rank; a block's full weights are
-        assembled in one of two ring buffers right before it runs — by copy-engine pulls from the peers' shards on one node, by
-        an NCCL all-gather otherwise (sharding.py).  Call after the weights are loaded.
-        LoRA factors stay replicated; `state_dict()` then only carries the replicated tensors and the LoRA parameters."""
-        from .sharding import ShardedBlocks
-        if self._sharded is not None:
-            return self
-        stacked = {k: self.w[k] for k in self._PER_LAYER}
-        self._sharded = ShardedBlocks(stacked, self.L, group, gather=gather)
-        for k in self._PER_LAYER:
-            self.w[k] = self._sharded.rings[k]
-        del stacked
-        if torch.cuda.is_available():
-            torch.cuda.empty_cache()
-        return self
-
-    def _linear_table(self) -> dict:
-        D = self.D
-        dims = {"qkv": (D, D, 3), "out": (D, D, 1), "up": (D, 4 * D, 1), "down": (4 * D, D, 1)}
-        t = {}
-        for l in range(self.L):
-            for nm, (grp, s, slot) in _BLOCK_LINEARS.items():
-                d_in, d_out, n = dims[grp]
-                t[f"transformer_blocks.{l}.{nm}"] = ((l, grp), (s,), slot, d_in, d_out, n)
-        return t
-
-    # ------------------------------------------------------------------------------------------------ workspace
-    def _mod_table(self) -> dict:
-        t = {}
-        for l in range(self.L):
-            t[f"transformer_blocks.{l}.img_mod.1"] = ("dbl", 2 * l, 6)
-            t[f"transformer_blocks.{l}.txt_mod.1"] = ("dbl", 2 * l + 1, 6)
-        return t
+        return self._double_weight_views(out)
 
     def _embed_table(self) -> dict:
         return {"img_in": ("img_in", 0, self.C_in), "txt_in": ("txt_in", 1, self.J)}
 
+    # ------------------------------------------------------------------------------------------------ workspace
     def _workspace(self, B, T, Limg, train: bool):
         def build():
             ws = self._alloc_common({}, B, T, Limg, train, self.L)
@@ -190,14 +141,6 @@ class QwenImageB200(FusedMMDiTBase):
         if key not in self._rope_cache:
             self._rope_cache[key] = qwen_rope_table(img_shapes, T, self.config.axes_dims_rope).to(self.dev)
         return self._rope_cache[key]
-
-    def _mods(self, ws, l):
-        """j -> (image view, text view) of the j-th D-wide modulation chunk of block l (shift1,scale1,gate1,shift2,scale2,gate2)."""
-        D = self.D
-
-        def f(j):
-            return tuple(ws["mods"][:, ((l * 2 + s) * 6 + j) * D: ((l * 2 + s) * 6 + j + 1) * D] for s in (0, 1))
-        return f
 
     # ------------------------------------------------------------------------------------------------ forward
     def _rope_multi(self, img_shapes, T, Limg, txt_lens=None):
@@ -251,8 +194,7 @@ class QwenImageB200(FusedMMDiTBase):
         lib.timestep_sinusoid(t32, 1000.0, ws["sin"])
         lib.gemv_act(ws["sin"], w["t1_w"], w["t1_b"], ws["t1"], act=0)
         lib.gemv_act(ws["t1"], w["t2_w"], w["t2_b"], ws["temb"], act=1)
-        sh = self._sharded
-        if sh is None:  # all 2L modulation linears in one launch
+        if self._sharded is None:  # all 2L modulation linears in one launch; sharded weights produce them block by block
             lib.gemv_act(ws["temb"], w["mod_w"].view(L * 2 * 6 * D, D), w["mod_b"].view(-1), ws["mods"], act=1)
             self._mod_lora_fwd(ws, ws["temb"])
         lib.gemv_act(ws["temb"], w["norm_out_w"], w["norm_out_b"], ws["fmod"], act=1)
@@ -261,83 +203,25 @@ class QwenImageB200(FusedMMDiTBase):
         self._embed_fwd(ws, "img_in", 0, hs, X0[Mt:])
         lib.rmsnorm_rows(encoder_hidden_states.to(BF).reshape(Mt, self.J), w["txt_norm_w"], ws["txt_n"])
         self._embed_fwd(ws, "txt_in", 1, ws["txt_n"], X0[:Mt])
-        # --- blocks
-        for l in range(L):
-            Xin, Xout = (ws["X"][l], ws["X"][l + 1]) if train else (ws["X"][l & 1], ws["X"][(l + 1) & 1])
-            if sh is not None:  # block l's weights arrive by all-gather (block l+1's gather starts now, on the side stream)
-                sh.acquire(l, then_prefetch=l + 1)
-                lib.gemv_act(ws["temb"], w["mod_w"][l].view(2 * 6 * D, D), w["mod_b"][l].view(-1),
-                             ws["mods"][:, l * 12 * D:(l + 1) * 12 * D], act=1)
-                self._mod_lora_fwd(ws, ws["temb"], ("dbl", (2 * l, 2 * l + 1)))
-            self._double_fwd(ws, l, Xin, Xout, ws["dbl"][l if train else 0], self._mods(ws, l))
-            if sh is not None:
-                sh.release(l)
-        Xl = ws["X"][L] if train else ws["X"][L & 1]
-        ws["Xlast"] = Xl
-        # --- output head: AdaLayerNormContinuous (scale, shift) + proj_out, image stream only
-        lib.ln_modulate_fwd(Xl[Mt:], ws["hn"], ws["fmod"][:, D:], ws["fmod"][:, :D], Limg, ws["fstats"][0], ws["fstats"][1])
-        lib.gemm([lib.gemm_problem(ws["hn"], w["proj_out_w"], ws["pred"], bias=w["proj_out_b"])], self.C_out, D)
-        return ws["pred"].view(B, Limg, self.C_out)
-
-    # ------------------------------------------------------------------------------------------------ backward
-    def _backward_impl(self, dpred):
-        """dpred: [B*Limg, C_out] bf16 gradient of the loss wrt the prediction; accumulates LoRA grads into self.G32."""
-        ws = self._ws
-        assert ws is not None and self._ws_key[3], "backward needs a training-mode forward first"
-        Limg, Mt = ws["Limg"], ws["Mt"]
-        D, L, w = self.D, self.L, self.w
-        self._mod_grad_buffers(ws)
-        # --- head: proj_out dgrad -> final AdaLN backward.  Text rows of the last block output receive no gradient.
-        lib.gemm([lib.gemm_problem(dpred, w["proj_out_w"], ws["dhn"])], D, self.C_out, trans_b=True)
-        dX = ws["dX"][L & 1]
-        dX[:Mt].zero_()
-        ws["dY"][:Mt].zero_()
-        lib.ln_modulate_bwd(ws["dhn"], ws["Xlast"][Mt:], ws["fstats"][0], ws["fstats"][1], ws["fmod"][:, :D], Limg, dX[Mt:],
-                            gate=self._mods(ws, L - 1)(5)[0], dx_gated=ws["dY"][Mt:])
-        sh = self._sharded
-        for l in range(L - 1, -1, -1):
-            dXn = ws["dX"][l & 1]
-            if sh is not None:
-                sh.acquire(l, then_prefetch=l - 1)
-            self._double_bwd(ws, l, ws["X"][l], dX, dXn, ws["dbl"][l], self._mods(ws, l),
-                             self._mods(ws, l - 1)(5) if l > 0 else None)
-            if sh is not None:
-                sh.release(l)
-            dX = dXn
-        self._mod_lora_bwd(ws)
-        self._embed_bwd(ws, "img_in", 0, dX)
-        self._embed_bwd(ws, "txt_in", 1, dX)
+        return self._blocks_and_head_fwd(ws, train)
 
     # ------------------------------------------------------------------------------------------------ public API
     def forward(self, hidden_states, encoder_hidden_states=None, encoder_hidden_states_mask=None, timestep=None,
                 img_shapes=None, txt_seq_lens=None, guidance=None, attention_kwargs=None, return_dict=False):
         """Same signature as the reference model.  With grad enabled and an adapter attached the result carries
         autograd history to the LoRA parameters (custom Function around the fused backward)."""
-        if torch.is_inference_mode_enabled():
-            # the reference's validation loop runs under torch.inference_mode() (qwen_image_edit_trainer.py:1219): workspaces and cached
-            # tables allocated there would be inference tensors, which later no_grad / training calls may not update in place
-            with torch.inference_mode(False), torch.no_grad():
-                return self.forward(hidden_states, encoder_hidden_states, encoder_hidden_states_mask, timestep, img_shapes, txt_seq_lens,
-                                    guidance, attention_kwargs, return_dict)
-        nested = isinstance(img_shapes[0], (list, tuple)) and isinstance(img_shapes[0][0], (list, tuple))
-        multi = nested and any(list(map(tuple, sh)) != list(map(tuple, img_shapes[0])) for sh in img_shapes)
-        txt_len = None
-        if multi and encoder_hidden_states_mask is not None:  # the mask is only honoured in multi-resolution mode (like the reference)
-            txt_len = encoder_hidden_states_mask.to(self.dev).sum(dim=1).to(torch.int32)
-        args = (hidden_states, encoder_hidden_states, timestep, img_shapes)
-        if multi:
-            args = args + (txt_len,)
-            if self.rope_placement == "reference":
-                if txt_seq_lens is None:
-                    raise ValueError("rope_placement='reference' needs txt_seq_lens (one text length per sample), as the reference's forward takes it")
-                args = args + (tuple(int(n) for n in txt_seq_lens),)
-        if torch.is_grad_enabled() and self._lora_params:
-            out = ModelFn.apply(self, args, *self._lora_params.values())
-        else:
-            out = self._infer(args).clone()
-        kv = self._ws.get("kv_len")
-        if kv is not None:  # padded image rows of a multi-resolution batch are returned as exact zeros (test_qwen_custom.py:672-692)
-            T = encoder_hidden_states.shape[1]
-            valid = torch.arange(out.shape[1], device=out.device)[None, :] < (kv[:, None] - T)
-            out = out * valid[..., None].to(out.dtype)
-        return (out,)
+        def make_args():
+            nested = isinstance(img_shapes[0], (list, tuple)) and isinstance(img_shapes[0][0], (list, tuple))
+            multi = nested and any(list(map(tuple, sh)) != list(map(tuple, img_shapes[0])) for sh in img_shapes)
+            txt_len = None
+            if multi and encoder_hidden_states_mask is not None:  # the mask is only honoured in multi-resolution mode (like the reference)
+                txt_len = encoder_hidden_states_mask.to(self.dev).sum(dim=1).to(torch.int32)
+            args = (hidden_states, encoder_hidden_states, timestep, img_shapes)
+            if multi:
+                args = args + (txt_len,)
+                if self.rope_placement == "reference":
+                    if txt_seq_lens is None:
+                        raise ValueError("rope_placement='reference' needs txt_seq_lens (one text length per sample), as the reference's forward takes it")
+                    args = args + (tuple(int(n) for n in txt_seq_lens),)
+            return args
+        return self._forward_tail(make_args)

@@ -168,15 +168,13 @@ class ShardedBlocks:
             self.shard = None
             self._peer_buf.free()
 
-    def acquire(self, l: int, then_prefetch=None):
-        """Make block l's weights valid for kernels on the current stream; optionally start fetching the next block."""
+    def acquire(self, l: int):
+        """Make block l's weights valid for kernels on the current stream."""
         self.prefetch(l)
         s = l & 1
         if self.cuda and self.pending[s]:
             torch.cuda.current_stream().wait_event(self.ready[s])
             self.pending[s] = False
-        if then_prefetch is not None:
-            self.prefetch(then_prefetch)
 
     def release(self, l: int):
         """The kernels of block l have been enqueued on the current stream; its slot may be refilled once they finish."""

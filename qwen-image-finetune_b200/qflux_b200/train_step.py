@@ -15,6 +15,7 @@ import torch
 import torch.distributed as dist
 
 from . import lib
+from .mmdit_base import GraphCache
 from .qwen_model import BF, QwenImageB200
 
 
@@ -43,89 +44,68 @@ def token_weights_and_norm(kind, B, L, C, weighting=None, attention_mask=None, e
     raise ValueError(f"unknown loss kind {kind!r}")
 
 
-class _Accumulation:
-    """Gradient accumulation (`accelerator.accumulate(...)` around training_step, base_trainer.py:518-533, train.gradient_accumulation_steps):
-    micro-steps add into the same flat fp32 LoRA gradient; the exchange + clip + optimizer step run on the last one with the mean over
-    micro-steps and ranks (accelerate divides the loss by the number of accumulation steps)."""
+class _FusedStep:
+    """What the step recipes share: loss weights, the fused loss + backward tail of `_run`, the autograd entry (`compute_loss`) and
+    the fast path (`train_step`) with gradient accumulation (`accelerator.accumulate(...)` around training_step,
+    base_trainer.py:518-533, train.gradient_accumulation_steps): micro-steps add into the same flat fp32 LoRA gradient; the exchange +
+    clip + optimizer step run on the last one with the mean over micro-steps and ranks (accelerate divides the loss by the number of
+    accumulation steps).
 
-    MAX_GRAPHS = 16
+    The fused step is ~1,300 (Qwen) to ~3,400 (FLUX with the YAML target set) kernel launches issued from Python through ctypes:
+    170-210 ms of host time per step, close to (FLUX: above) the device time.  All of it is shape-static, so `train_step` runs it
+    through a CUDA-graph cache (mmdit_base.GraphCache) keyed on the input signature and on whether the micro-step accumulates; every
+    replayed step is a handful of small copies plus one graph launch.  The exchange + clip + optimizer stay outside (NCCL, and the
+    optimizer's step count is a kernel argument)."""
 
-    def _init_accumulation(self, steps: int, use_cuda_graph: bool = True):
-        self.gradient_accumulation_steps, self._micro = max(1, int(steps)), 0
-        self.use_cuda_graph, self._graphs = bool(use_cuda_graph), {}
+    def __init__(self, dit, loss_kind: str = "mse", fg: float = 2.0, bg: float = 1.0, max_grad_norm: float = 1.0,
+                 gradient_accumulation_steps: int = 1, use_cuda_graph: bool = True):
+        self.dit, self.loss_kind, self.fg, self.bg, self.max_grad_norm = dit, loss_kind, fg, bg, max_grad_norm
+        self._ones = {}
+        self._accumulating = False
+        self.gradient_accumulation_steps, self._micro = max(1, int(gradient_accumulation_steps)), 0
+        self.use_cuda_graph, self._graphs = bool(use_cuda_graph), GraphCache(16, "the fused step")
 
-    # ------------------------------------------------------------------------------------------------ CUDA graph of fwd + loss + bwd
-    # The fused step is ~1,300 (Qwen) to ~3,400 (FLUX with the YAML target set) kernel launches issued from Python through ctypes:
-    # 170-210 ms of host time per step, close to (FLUX: above) the device time.  All of it is shape-static, so the second step of a given
-    # shape is captured into a CUDA graph (inputs copied into static buffers, kernel arguments — TMA descriptors included — baked in) and
-    # every later step is a handful of small copies plus one graph launch.  The exchange + clip + optimizer stay outside (NCCL, and the
-    # optimizer's step count is a kernel argument).  Sharded frozen weights (side-stream all-gathers) run eagerly.
-    @staticmethod
-    def _sig(a):
-        if torch.is_tensor(a):
-            return ("t", tuple(a.shape), str(a.dtype))
-        if isinstance(a, (tuple, list)):
-            return tuple(_Accumulation._sig(x) for x in a)
-        return repr(a)
+    def _dense_loss_weights(self, B, L, C, edit_mask):
+        """(w [B, L] fp32 on the device, norm) of a batch whose samples share one resolution."""
+        dev = self.dit.dev
+        if self.loss_kind == "mse" and edit_mask is None:
+            if (B, L) not in self._ones:
+                self._ones[(B, L)] = torch.ones(B, L, device=dev)
+            return self._ones[(B, L)], 1.0 / (B * L * C)
+        w, norm = token_weights_and_norm(self.loss_kind, B, L, C, None, None, None if edit_mask is None else edit_mask.to(dev),
+                                         self.fg, self.bg)
+        return w.to(dev).contiguous(), norm
 
-    def _run_maybe_graphed(self, args):
+    def _var_lengths(self, shapes, L):
+        """Pad-to-max multi-resolution batch: img_shapes holds one list of latent (frame, h, w) per sample, target first, then the
+        controls.  Returns (target tokens lt, control tokens lc (host lists), padded length Ltot, Lt, Lc (int32 [B] on the device),
+        target-token mask [B, L] (host fp32))."""
+        dev = self.dit.dev
+        lt = [f * h * w for f, h, w in (sh[0] for sh in shapes)]
+        lc = [sum(f * h * w for f, h, w in sh[1:]) for sh in shapes]
+        Lt = torch.tensor(lt, dtype=torch.int32).to(dev, non_blocking=True)
+        Lc = torch.tensor(lc, dtype=torch.int32).to(dev, non_blocking=True)
+        amask = (torch.arange(L)[None, :] < torch.tensor(lt)[:, None]).float()
+        return lt, lc, max(a + b for a, b in zip(lt, lc)), Lt, Lc, amask
+
+    def _loss_and_backward(self, pred, x0, noise, w, norm):
+        """Tail of `_run`: flow-matching loss and its gradient, then the fused backward into the flat LoRA gradient (zeroed first unless
+        this micro-step accumulates).  Returns the loss (a workspace scalar)."""
         m = self.dit
-        if not self.use_cuda_graph or m._sharded is not None or not torch.cuda.is_available() or not m.dev.type == "cuda":
-            return self._run(*args)
-        key = (self._sig(args), self._accumulating)
-        ent = self._graphs.pop(key, None)
-        if ent is not None:
-            self._graphs[key] = ent  # most recently used last
-        if ent is None:  # first step of this shape: eager (allocates the workspace, RoPE tables, split-K scratch, sets kernel attributes)
-            while len(self._graphs) >= self.MAX_GRAPHS:  # bucketed multi-resolution training: keep the most recent shape combinations only
-                self._graphs.pop(next(iter(self._graphs)))   # (every captured graph owns a private memory pool)
-            self._graphs[key] = "warm"
-            return self._run(*args)
-        if ent != "warm" and ent["ws"] is not m._ws and not m._activate_ws(ent["ws"], ent["ws_key"]):
-            ent = "warm"  # the model dropped the workspace this graph was recorded on (another training shape ran in between): record again
-        if ent == "warm":
-            static = self._clone_args(args)
-            torch.cuda.synchronize()
-            g = torch.cuda.CUDAGraph()
-            n0 = lib.LAUNCHES
-            try:
-                with torch.cuda.graph(g):
-                    loss = self._run(*static)
-            except Exception as e:  # something on this path is not capturable: say so once and stay eager (never silently wrong)
-                import warnings
-                warnings.warn(f"qflux_b200: CUDA-graph capture of the fused step failed ({type(e).__name__}: {e}); running eagerly")
-                torch.cuda.synchronize()
-                self.use_cuda_graph = False
-                lib.LAUNCHES = n0
-                return self._run(*args)
-            # `keep`: per-shape tables the captured kernels point at (RoPE, key lengths, ragged row bands) live in bounded caches of the model —
-            # the graph must keep them alive after they are evicted there
-            ent = dict(graph=g, static=static, loss=loss, launches=lib.LAUNCHES - n0, ws=m._ws, ws_key=m._ws_key,
-                       keep=tuple(m._ws.get(k) for k in ("rope", "kv_len", "txt_len", "bands")))
-            lib.LAUNCHES = n0  # capture launches nothing
-            self._graphs[key] = ent
-        self._copy_args(ent["static"], args)
-        ent["graph"].replay()
-        lib.LAUNCHES += ent["launches"]
-        return ent["loss"]
+        ws = m._ws
+        lib.flow_loss(pred, x0, noise, w, norm, ws["loss"], ws["dpred"])
+        if not self._accumulating:
+            m.G32.zero_()
+        m._backward_impl(ws["dpred"])
+        return ws["loss"]
 
-    @staticmethod
-    def _clone_args(args):
-        return tuple(a.clone() if torch.is_tensor(a) else (_Accumulation._clone_args(a) if isinstance(a, tuple) else a) for a in args)
-
-    @staticmethod
-    def _copy_args(static, args):
-        for s_, a in zip(static, args):
-            if torch.is_tensor(s_):
-                if s_.data_ptr() != a.data_ptr():
-                    s_.copy_(a, non_blocking=True)
-            elif isinstance(s_, tuple):
-                _Accumulation._copy_args(s_, a)
+    def _autograd_loss(self, args):
+        return _StepFn.apply(self, args, *self.dit._lora_params.values())
 
     def _fused_micro_step(self, args, optimizer):
         self._accumulating = self._micro > 0  # read by _run: keep the gradient of the earlier micro-steps
-        loss = self._run_maybe_graphed(args).clone()  # the workspace scalar is overwritten by the next step
-        self.dit._fwd_gen += 1                         # (a graph replay does not pass through _forward_impl)
+        loss = self._graphs.run(self.dit, self._run, args, tag=self._accumulating, enabled=self.use_cuda_graph)
+        loss = loss.clone()  # the workspace scalar is overwritten by the next step
         self._accumulating = False
         self._micro += 1
         if self._micro >= self.gradient_accumulation_steps:
@@ -174,15 +154,12 @@ class _StepFn(torch.autograd.Function):
         return (None, None) + grads
 
 
-class QwenImageEditStep(_Accumulation):
+class QwenImageEditStep(_FusedStep):
     def __init__(self, dit: QwenImageB200, loss_kind: str = "mse", fg: float = 2.0, bg: float = 1.0,
                  num_train_timesteps: int = 1000, max_grad_norm: float = 1.0, gradient_accumulation_steps: int = 1,
                  use_cuda_graph: bool = True):
-        self.dit, self.loss_kind, self.fg, self.bg = dit, loss_kind, fg, bg
-        self.num_train_timesteps, self.max_grad_norm = num_train_timesteps, max_grad_norm
-        self._ones = {}
-        self._accumulating = False
-        self._init_accumulation(gradient_accumulation_steps, use_cuda_graph)
+        super().__init__(dit, loss_kind, fg, bg, max_grad_norm, gradient_accumulation_steps, use_cuda_graph)
+        self.num_train_timesteps = num_train_timesteps
 
     # --------------------------------------------------------------------------------------------- internals
     def _sigmas(self, B, u=None):
@@ -204,12 +181,7 @@ class QwenImageEditStep(_Accumulation):
             packed = torch.empty(B, Ltot, C, device=m.dev, dtype=BF)
             lib.flow_noisy_input_var(image_latents, noise, control_latents, sigma, Lt, Lc, packed)
             pred = m._forward_impl(packed, prompt_embeds, sigma, img_shapes, txt_len, train=True)
-        ws = m._ws
-        lib.flow_loss(pred, image_latents, noise, w, norm, ws["loss"], ws["dpred"])
-        if not self._accumulating:
-            m.G32.zero_()
-        m._backward_impl(ws["dpred"])
-        return ws["loss"]
+        return self._loss_and_backward(pred, image_latents, noise, w, norm)
 
     def _prepare(self, embeddings, noise, u):
         m = self.dit
@@ -229,33 +201,19 @@ class QwenImageEditStep(_Accumulation):
         if multi:
             # pad-to-max multi-resolution batch (SURVEY.md §8a a4/a11): token counts come from the latent-space shapes (host
             # metadata), the loss is AttentionMaskMseLoss over the valid target tokens (attention_mask_loss.py:146-226)
-            lt = [sh[0][0] * sh[0][1] * sh[0][2] for sh in shapes]
-            lc = [sum(f * h * w_ for (f, h, w_) in sh[1:]) for sh in shapes]
-            Ltot = max(a + b for a, b in zip(lt, lc))
-            Lt = torch.tensor(lt, dtype=torch.int32).to(dev, non_blocking=True)
-            Lc = torch.tensor(lc, dtype=torch.int32).to(dev, non_blocking=True)
+            lt, lc, Ltot, Lt, Lc, amask = self._var_lengths(shapes, L)
             mask = embeddings.get("prompt_embeds_mask")
             txt_len = None if mask is None else mask.to(dev).sum(dim=1).to(torch.int32)
-            amask = (torch.arange(L)[None, :] < torch.tensor(lt)[:, None]).float()
             w = amask if edit_mask is None else amask * (edit_mask.float().cpu() * self.fg + (1 - edit_mask.float().cpu()) * self.bg)
             norm = 1.0 / (C * (float(sum(lt)) + 1e-12))
             return (x0, ctrl, pe, shapes, noise.to(dev, BF), sigma, w.to(dev).contiguous(), norm, (Lt, Lc, Ltot, txt_len))
-        if self.loss_kind == "mse" and edit_mask is None:
-            key = (B, L)
-            if key not in self._ones:
-                self._ones[key] = torch.ones(B, L, device=dev)
-            w, norm = self._ones[key], 1.0 / (B * L * C)
-        else:
-            w, norm = token_weights_and_norm(self.loss_kind, B, L, C, None, None,
-                                             None if edit_mask is None else edit_mask.to(dev), self.fg, self.bg)
-            w = w.to(dev).contiguous()
+        w, norm = self._dense_loss_weights(B, L, C, edit_mask)
         return (x0, ctrl, pe, shapes, noise.to(dev, BF), sigma, w, norm)
 
     # --------------------------------------------------------------------------------------------- public
     def compute_loss(self, embeddings: dict, noise=None, u=None) -> torch.Tensor:
         """Drop-in for `Trainer._compute_loss(embeddings)`: scalar loss whose `.backward()` fills the LoRA `.grad`s."""
-        args = self._prepare(embeddings, noise, u)
-        return _StepFn.apply(self, args, *self.dit._lora_params.values())
+        return self._autograd_loss(self._prepare(embeddings, noise, u))
 
     @torch.no_grad()
     def train_step(self, embeddings: dict, optimizer=None, noise=None, u=None):
@@ -264,17 +222,10 @@ class QwenImageEditStep(_Accumulation):
         return self._fused_micro_step(self._prepare(embeddings, noise, u), optimizer)
 
 
-class FluxKontextStep(_Accumulation):
+class FluxKontextStep(_FusedStep):
     """Mirror of `FluxKontextLoraTrainer._compute_loss_shared_mode`
     (/root/reference/src/qflux/trainer/flux_kontext_trainer.py:494-577): t ~ U(0,1) in bf16 on the device, x_t = (1-t) x0 + t eps,
     ids = [target ids ; control ids], guidance = 1 when the model has guidance embeddings, target = eps - x0, MSE."""
-
-    def __init__(self, dit, loss_kind: str = "mse", fg: float = 2.0, bg: float = 1.0, max_grad_norm: float = 1.0,
-                 gradient_accumulation_steps: int = 1, use_cuda_graph: bool = True):
-        self.dit, self.loss_kind, self.fg, self.bg, self.max_grad_norm = dit, loss_kind, fg, bg, max_grad_norm
-        self._ones = {}
-        self._accumulating = False
-        self._init_accumulation(gradient_accumulation_steps, use_cuda_graph)
 
     @staticmethod
     def latent_image_ids(h2, w2, device, first=0.0):
@@ -303,14 +254,7 @@ class FluxKontextStep(_Accumulation):
         if shapes is not None and any(list(map(tuple, sh)) != list(map(tuple, shapes[0])) for sh in shapes):
             return self._prepare_multi(embeddings, x0, ctrl, pe, pooled, noise.to(dev, BF), t, edit_mask, shapes)
         ids = torch.cat([embeddings["image_ids"].to(dev), embeddings["control_ids"].to(dev)], dim=0)
-        if self.loss_kind == "mse" and edit_mask is None:
-            if (B, L) not in self._ones:
-                self._ones[(B, L)] = torch.ones(B, L, device=dev)
-            w, norm = self._ones[(B, L)], 1.0 / (B * L * C)
-        else:
-            w, norm = token_weights_and_norm(self.loss_kind, B, L, C, None, None, None if edit_mask is None else edit_mask.to(dev),
-                                             self.fg, self.bg)
-            w = w.to(dev).contiguous()
+        w, norm = self._dense_loss_weights(B, L, C, edit_mask)
         guidance = torch.ones(B, device=dev) if m.config.guidance_embeds else None
         return (x0, ctrl, pe, pooled, embeddings["text_ids"].to(dev), ids, noise.to(dev, BF), t, guidance, w, norm)
 
@@ -323,19 +267,14 @@ class FluxKontextStep(_Accumulation):
         m, dev = self.dit, self.dit.dev
         B, L, C = x0.shape
         T = pe.shape[1]
-        lt = [sh[0][1] * sh[0][2] for sh in shapes]
-        lc = [sum(h * w_ for (_, h, w_) in sh[1:]) for sh in shapes]
-        Ltot = max(a + b for a, b in zip(lt, lc))
+        lt, lc, Ltot, Lt, Lc, amask = self._var_lengths(shapes, L)
         ids = torch.zeros(B, Ltot, 3)
         for b, sh in enumerate(shapes):
             parts = [self.latent_image_ids(sh[0][1], sh[0][2], "cpu", 0.0)]
             parts += [self.latent_image_ids(h, w_, "cpu", float(j + 1)) for j, (_, h, w_) in enumerate(sh[1:])]
             cat = torch.cat(parts, dim=0)
             ids[b, : cat.shape[0]] = cat
-        Lt = torch.tensor(lt, dtype=torch.int32).to(dev, non_blocking=True)
-        Lc = torch.tensor(lc, dtype=torch.int32).to(dev, non_blocking=True)
         kv_len = torch.tensor([T + a + b for a, b in zip(lt, lc)], dtype=torch.int32).to(dev, non_blocking=True)
-        amask = (torch.arange(L)[None, :] < torch.tensor(lt)[:, None]).float()
         w = amask
         if edit_mask is not None and self.loss_kind != "mse":
             em = edit_mask.float().cpu()
@@ -359,16 +298,10 @@ class FluxKontextStep(_Accumulation):
             packed = torch.empty(B, Ltot, C, device=m.dev, dtype=BF)
             lib.flow_noisy_input_var(x0, noise, ctrl, t.float().contiguous(), Lt, Lc, packed)
             pred = m._forward_impl(packed, pe, pooled, t, ids, text_ids, guidance, kv_len, train=True, valid_rows=valid_rows)
-        ws = m._ws
-        lib.flow_loss(pred, x0, noise, w, norm, ws["loss"], ws["dpred"])
-        if not self._accumulating:
-            m.G32.zero_()
-        m._backward_impl(ws["dpred"])
-        return ws["loss"]
+        return self._loss_and_backward(pred, x0, noise, w, norm)
 
     def compute_loss(self, embeddings: dict, noise=None, t=None) -> torch.Tensor:
-        args = self._prepare(embeddings, noise, t)
-        return _StepFn.apply(self, args, *self.dit._lora_params.values())
+        return self._autograd_loss(self._prepare(embeddings, noise, t))
 
     @torch.no_grad()
     def train_step(self, embeddings: dict, optimizer=None, noise=None, t=None):

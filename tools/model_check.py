@@ -220,7 +220,7 @@ def graph_replay():
     l_new_g = float(graphed.train_step(emb, noise=noise2, u=x["u"]))
     res["qwen_new_inputs"] = max(abs(l_new_e - l_new_g), rel_l2(m.G32, g_new_e))
     assert abs(l_new_e - l_e) > 1e-3, "the second input set must actually differ"
-    assert len(graphed._graphs) == 1 and isinstance(next(iter(graphed._graphs.values())), dict), "no graph was captured"
+    assert len(graphed._graphs.entries) == 1 and graphed._graphs.captured() == 1, "no graph was captured"
     # FLUX with the YAML target regex
     orc, mf = build_flux_pair(targets=FLUX_YAML_TARGETS, r=4)
     g = torch.Generator(device="cuda").manual_seed(3)
@@ -236,7 +236,7 @@ def graph_replay():
     ls = [float(fg.train_step(embf, noise=nz, t=t)) for _ in range(3)]
     res["flux_loss"] = max(abs(le - v) for v in ls)
     res["flux_grad"] = rel_l2(mf.G32, ge)
-    assert len(fg._graphs) == 1 and isinstance(next(iter(fg._graphs.values())), dict), "no FLUX graph was captured"
+    assert len(fg._graphs.entries) == 1 and fg._graphs.captured() == 1, "no FLUX graph was captured"
     res["err"] = max(res.values())
     return res
 
@@ -267,7 +267,7 @@ def grad_accum():
                     step.train_step(emb, opt, noise=x["noise"][b:b + 1], u=x["u"][b:b + 1])
                 gs.append(m.G32.clone() / 2)  # the accumulator holds the SUM over micro-steps; the optimizer divides
             assert opt.step_count == 3
-            n_graphs = sum(isinstance(v, dict) for v in step._graphs.values())
+            n_graphs = step._graphs.captured()
             assert n_graphs == 2, f"expected one graph per micro-step kind, got {n_graphs}"
         out[mode] = (gs, [p.detach().float().clone() for p in m.parameters()])
     res = dict(grad=max(rel_l2(a, b) for a, b in zip(out["accum"][0], out["big"][0])))
@@ -342,7 +342,7 @@ def infer_graph_replay():
         worst = max(worst, max(float((a.float() - b.float()).abs().max()) for a, b in zip(got, ref)))
         if rep == 2:
             step.train_step(emb, noise=x["noise"], u=x["u"])
-    n_graphs = sum(isinstance(v, dict) for v in m._infer_graphs.values())
+    n_graphs = m._infer_graphs.captured()
     assert n_graphs == 2, f"expected two captured inference graphs, got {n_graphs}"
     # the sampling loop end to end, graphed vs eager
     e = dict(latents=rn(2, 16, 64), control_latents=x["control_latents"], prompt_embeds=pe_a, prompt_embeds_mask=torch.ones(2, 24, dtype=torch.int64, device="cuda"),
