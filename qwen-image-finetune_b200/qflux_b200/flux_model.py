@@ -150,22 +150,14 @@ class FluxB200(FusedMMDiTBase):
 
     # ------------------------------------------------------------------------------------------------ workspace
     def _workspace(self, B, T, Limg, train: bool):
-        def build():
-            ws = self._alloc_common({}, B, T, Limg, train, self.L, self.Ls)
-            D = self.D
-            e = lambda *s, dt=BF: torch.empty(*s, device=self.dev, dtype=dt)
-            for k in ("sin", "gsin"):
-                ws[k] = e(B, 256)
-            for k in ("e1", "temb", "gemb", "pemb"):
-                ws[k] = e(B, D)
-            ws["mods"] = e(B, self.L * 2 * 6 * D)
-            ws["smods"] = e(B, max(self.Ls, 1) * 3 * D)
-            ws["fmod"] = e(B, 2 * D)
-            return ws
-        return self._get_workspace((B, T, Limg, train), build)
+        D = self.D
+        extra = [(k, (B, 256)) for k in ("sin", "gsin")] + [(k, (B, D)) for k in ("e1", "temb", "gemb", "pemb")]
+        extra += [("mods", (B, self.L * 2 * 6 * D)), ("smods", (B, max(self.Ls, 1) * 3 * D)), ("fmod", (B, 2 * D))]
+        return self._get_workspace((B, T, Limg, train), lambda: self._alloc_common({}, B, T, Limg, train, self.L, self.Ls, extra=extra))
 
     # ------------------------------------------------------------------------------------------------ single block
-    def _single_fwd(self, ws, l, Xin, Xout, save):
+    def _single_fwd(self, ws, l, Xin, Xout, save, recompute=False):
+        """recompute: as in `_double_fwd` — proj_out only runs when its un-gated output feeds the AdaLN-LoRA gate gradient."""
         D, w = self.D, self.w
         T, Mt = ws["T"], ws["Mt"]
         st, qkv, O, h, u = save["stats"], save["qkv"], save["O"], save["h"], save["u"]
@@ -177,8 +169,9 @@ class FluxB200(FusedMMDiTBase):
                                   round_mid=False)
         lib.attn_fwd(ws["Q"], ws["K"], ws["V"], O[:Mt], O[Mt:], T, save["lse"], kv_len=ws.get("kv_len"), txt_len=ws.get("txt_len"))
         # x = x + gate * proj_out(cat[attn, gelu(mlp)]): attention wrote columns [0, D) and the GELU epilogue [D, 5D) of save["cat"]
-        self._grouped(ws, l, "s_out", save["cat"], Xout, D, 5 * D, lib.EPI_RESID_GATE, resid=Xin, gate=self._smod(ws, l, 2),
-                      out2=save.get("y_out"))
+        if not recompute or self._keeps_gate_out(l, "sgl"):
+            self._grouped(ws, l, "s_out", save["cat"], Xout, D, 5 * D, lib.EPI_RESID_GATE, resid=Xin, gate=self._smod(ws, l, 2),
+                          out2=save.get("y_out"))
 
     def _single_bwd(self, ws, l, Xin, dX, dXn, save, prev_gate):
         D, w = self.D, self.w

@@ -15,6 +15,7 @@ import math
 import os
 import re
 import warnings
+from typing import NamedTuple
 
 import torch
 import torch.nn as nn
@@ -24,6 +25,49 @@ from . import lib
 BF = torch.bfloat16
 PAD = 64  # LoRA rank is padded to one 64-wide k-block
 DEFAULT_TARGETS = ("to_q", "to_k", "to_v", "to_out.0")  # /root/reference/src/qflux/data/config.py:315
+# Device memory left free when the training workspace is planned (the default activation limit is the free device memory minus this):
+# what a step allocates after its workspace.  Measured with tools/recompute_bench.py on an H100 80GB HBM3 (400 W), every Qwen-Image-Edit,
+# Edit-Plus and FLUX-Kontext point: the step's peak exceeded "allocated when planned + workspace" by at most 0.36 GiB (the captured
+# step graph's pool, step temporaries) and the allocator's reserved memory by at most 0.93 GiB.  The rest of the 4 GiB is left for
+# what that run did not allocate after its workspace: fused-AdamW moments of an optimizer built after the first step and the no-grad
+# workspaces of a validation pass (a few hundred MB each, up to three).
+ACTIVATION_HEADROOM = 4 << 30
+
+
+class ActivationPlan(NamedTuple):
+    """Which blocks of the training workspace keep their saved tensors (DESIGN.md §3).
+    recompute: global block indices (double blocks first, then single blocks) that keep only their input X[blk] — the backward
+    re-runs their forward into a scratch dict right before their backward; bytes: planned workspace bytes; saved_bytes: how many
+    fewer bytes than keep-all; min_bytes: the bytes with every block recomputed; limit: the bytes the workspace was allowed
+    (None: unlimited)."""
+    recompute: tuple
+    bytes: int
+    saved_bytes: int
+    min_bytes: int
+    limit: int | None
+
+
+def plan_activation_memory(blocks, fixed: int, limit: int | None) -> ActivationPlan:
+    """blocks: one (kind, {saved entry: bytes}) per block in execution order; fixed: the workspace bytes every plan allocates.
+    Keep-all when it fits `limit`, else recompute the fewest blocks, taken from the end of the stack.  The recomputed blocks of a
+    kind share one scratch dict holding every entry any of them needs.  Raises QfxError when not even recomputing every block fits."""
+    n = len(blocks)
+
+    def total(k):
+        scratch = {}
+        for kind, ent in blocks[n - k:]:
+            s = scratch.setdefault(kind, {})
+            for name, b in ent.items():
+                s[name] = max(s.get(name, 0), b)
+        return fixed + sum(sum(e.values()) for _, e in blocks[:n - k]) + sum(sum(s.values()) for s in scratch.values())
+
+    keep_all, least = total(0), total(n)
+    for k in range(n + 1):
+        t = total(k)
+        if limit is None or t <= limit:
+            return ActivationPlan(tuple(range(n - k, n)), t, keep_all - t, least, limit)
+    raise lib.QfxError(f"the training workspace needs {least} bytes with the activations of every block recomputed, but only {limit} "
+                       f"bytes are available for it (keeping every block would take {keep_all}): use a smaller batch or free device memory")
 
 
 class LoraSite:
@@ -131,7 +175,8 @@ class FusedMMDiTBase(nn.Module):
         self._ws = self._ws_key = None
         self._train_ws, self._infer_ws = None, {}   # cached workspaces (see _get_workspace)
         self._rope_cache = {}
-        self.gradient_checkpointing = False  # accepted for interface compatibility; HBM holds the activations
+        self.gradient_checkpointing = False  # accepted for interface compatibility (see enable_gradient_checkpointing)
+        self._activation_limit = None  # bytes the training workspace may take; None: free device memory - ACTIVATION_HEADROOM
         self._sharded = None     # sharding.ShardedBlocks once shard_frozen_weights() has run
         self._bands_cache = {}   # (valid image rows per sample, Limg) -> lib.RowBands (ragged GEMM row bands)
         self._infer_graphs, self.use_cuda_graph_inference = GraphCache(8, "the inference forward"), True  # see _infer
@@ -194,7 +239,22 @@ class FusedMMDiTBase(nn.Module):
             self._mod_lora_fwd(ws, ws["temb"], ("sgl", (l,)))
 
     def enable_gradient_checkpointing(self, *args, **kwargs):
+        """Accepted for the reference trainer's `gradient_checkpointing: True`.  It selects nothing: the training workspace always
+        recomputes the activations of exactly those blocks whose saved tensors do not fit the device (`activation_plan`)."""
         self.gradient_checkpointing = True
+
+    def set_activation_memory_limit(self, nbytes: int | None):
+        """Bytes the training workspace may take (None: the free device memory when it is built, minus ACTIVATION_HEADROOM).
+        Drops the cached training workspace; the next training step plans and allocates it again under the new limit."""
+        self._activation_limit = None if nbytes is None else int(nbytes)
+        if self._train_ws is not None and self._ws is self._train_ws[1]:
+            self._ws = self._ws_key = None
+        self._train_ws = None
+
+    @property
+    def activation_plan(self) -> ActivationPlan | None:
+        """The plan of the current training workspace (None before the first training step)."""
+        return None if self._train_ws is None else self._train_ws[1]["plan"]
 
     def _apply(self, fn, recurse=True):
         """`dit.to(accelerator.device)` / `.cuda()` / `.bfloat16()` (base_trainer.py:388, qwen_image_edit_trainer.py:300-330) are accepted
@@ -658,11 +718,6 @@ class FusedMMDiTBase(nn.Module):
         lib.ln_modulate_bwd_pair(dy, x, mean, rstd, (scale[1], ws["T"], g[1]), (scale[0], ws["Limg"], g[0]), ws["Mt"], dx, dres=dres,
                                  dx_gated=dx_gated if gate else None)
 
-    def _alloc_lora_T(self, ws):
-        ws["loraT"] = {}
-        for (l, grp, s), site in self.sites.items():
-            ws["loraT"][(l, grp, s)] = torch.zeros(ws["Mi"] if s == 0 else ws["Mt"], site.n * PAD, device=self.dev, dtype=BF)
-
     def _lora_T(self, ws, l, grp, s, X):
         """T = scaling * X @ A_pad^T  for the site (None if the site has no adapter)."""
         site = self._site(l, grp, s)
@@ -818,7 +873,10 @@ class FusedMMDiTBase(nn.Module):
 
     # ------------------------------------------------------------------------------------------------ double-stream block
     # mods(j): j-th D-wide chunk (shift1, scale1, gate1, shift2, scale2, gate2) -> (img view, txt view), each [B, D]
-    def _double_fwd(self, ws, l, Xin, Xout, save, mods):
+    def _double_fwd(self, ws, l, Xin, Xout, save, mods, recompute=False):
+        """recompute: regenerate the saved tensors of block l for its backward.  The down projection is skipped then (its output,
+        the next block's input, is kept) unless its un-gated output feeds an AdaLN-LoRA gate gradient; it then rewrites Xout,
+        which no later step of the backward reads."""
         D = self.D
         T, Limg, Mt = ws["T"], ws["Limg"], ws["Mt"]
         st, qkv, O, xmid, u = save["stats"], save["qkv"], save["O"], save["xmid"], save["u"]
@@ -835,7 +893,8 @@ class FusedMMDiTBase(nn.Module):
         lib.ln_modulate_fwd_pair(xmid, ws["xm"], (mods(3)[1], mods(4)[1], T), (mods(3)[0], mods(4)[0], Limg), Mt, st[2], st[3])
         h = save.get("h", ws["h"])  # kept per block only when ff.net.2 carries LoRA (its input is needed for dA)
         self._grouped(ws, l, "up", ws["xm"], h, 4 * D, D, lib.EPI_GELU, out2=u)
-        self._grouped(ws, l, "down", h, Xout, D, 4 * D, lib.EPI_RESID_GATE, resid=xmid, gate=mods(5), out2=save.get("y_mlp"))
+        if not recompute or self._keeps_gate_out(l):
+            self._grouped(ws, l, "down", h, Xout, D, 4 * D, lib.EPI_RESID_GATE, resid=xmid, gate=mods(5), out2=save.get("y_mlp"))
 
     def _attn_bwd_core(self, ws, qkv, O, lse, wq_wk, save=None):
         """dO (head-major ws['dOj'] + ws['delta'], written by the out-projection dgrad: _dgrad_attn_out) -> dqkv (ws['dqkv']);
@@ -966,6 +1025,11 @@ class FusedMMDiTBase(nn.Module):
             prev = self._last_gate(ws, blk - 1) if blk > 0 else None
             if self._sharded is not None:
                 self._acquire(blk, blk - 1)
+            if blk in ws["plan"].recompute:  # regenerate the block's saved tensors into the scratch dict (its weights are resident now)
+                if blk < L:
+                    self._double_fwd(ws, blk, ws["X"][blk], ws["X"][blk + 1], ws["dbl"][blk], self._mods(ws, blk), recompute=True)
+                else:
+                    self._single_fwd(ws, blk - L, ws["X"][blk], ws["X"][blk + 1], ws["sgl"][blk - L], recompute=True)
             if blk < L:
                 self._double_bwd(ws, blk, ws["X"][blk], dX, dXn, ws["dbl"][blk], self._mods(ws, blk), prev)
             else:
@@ -978,53 +1042,99 @@ class FusedMMDiTBase(nn.Module):
             self._embed_bwd(ws, key, s, dX)
 
     # ------------------------------------------------------------------------------------------------ workspace pieces
-    def _alloc_common(self, ws, B, T, Limg, train, n_double, n_single=0):
-        D, H = self.D, self.H
-        Mt, Mi = B * T, B * Limg
-        M, S = Mt + Mi, T + Limg
-        e = lambda *s, dt=BF: torch.empty(*s, device=self.dev, dtype=dt)
-        ws.update(B=B, T=T, Limg=Limg, S=S, Mt=Mt, Mi=Mi, M=M)
-        nblk = n_double + n_single
-        ws["X"] = e(nblk + 1 if train else 2, M, D)
-        ws["xm"], ws["h"] = e(M, D), e(M, 4 * D)
-        ws["Q"], ws["K"], ws["V"] = e(B, H, S, 128), e(B, H, S, 128), e(B, H, S, 128)
-        nd = n_double if train else min(1, n_double)
-        ns = n_single if train else min(1, n_single)
-        ws["dbl"] = [dict(stats=e(4, M, dt=torch.float32), qkv=e(M, 3 * D), O=e(M, D), lse=e(B, H, S, dt=torch.float32),
-                          xmid=e(M, D), u=e(M, 4 * D)) for _ in range(nd)]
-        if train and self.keep_qkv:  # +4 x [M, D] per block in HBM instead of regenerating them in the backward
-            for blk in ws["dbl"]:
-                blk.update(Q=e(B, H, S, 128), K=e(B, H, S, 128), V=e(B, H, S, 128), xm1=e(M, D))
-        if train:
-            for l, blk in enumerate(ws["dbl"]):
-                if self._site(l, "down", 0) or self._site(l, "down", 1):
-                    blk["h"] = e(M, 4 * D)
-                rows = self.mod_sites.get("dbl", {}).get("rows", ())
-                if 2 * l in rows or 2 * l + 1 in rows:  # un-gated branch outputs, needed for d gate
-                    blk["y_attn"], blk["y_mlp"] = e(M, D), e(M, D)
+    def _keeps_gate_out(self, l, kind="dbl"):
+        """Block l's un-gated branch outputs are saved: an AdaLN linear of the block carries LoRA (they feed d gate)."""
+        rows = self.mod_sites.get(kind, {}).get("rows", ())
+        return (2 * l in rows or 2 * l + 1 in rows) if kind == "dbl" else l in rows
+
+    def _saved_entries(self, kind, blocks, B, S, train):
+        """[(group, name, shape, dtype)] of the saved dict serving `blocks` (indices of one block kind; every optional entry any of
+        them needs).  Allocation runs group by group over the dicts of a kind."""
+        D, H, M, f32 = self.D, self.H, B * S, torch.float32
+        if kind == "dbl":
+            ent = [(0, "stats", (4, M), f32), (0, "qkv", (M, 3 * D), BF), (0, "O", (M, D), BF), (0, "lse", (B, H, S), f32),
+                   (0, "xmid", (M, D), BF), (0, "u", (M, 4 * D), BF)]
+            if train and self.keep_qkv:  # +4 x [M, D] per block in HBM instead of regenerating them in the backward
+                ent += [(1, "Q", (B, H, S, 128), BF), (1, "K", (B, H, S, 128), BF), (1, "V", (B, H, S, 128), BF), (1, "xm1", (M, D), BF)]
+            if train and any(self._site(l, "down", 0) or self._site(l, "down", 1) for l in blocks):
+                ent.append((2, "h", (M, 4 * D), BF))  # the LoRA input of ff.net.2
+            if train and any(self._keeps_gate_out(l) for l in blocks):  # un-gated branch outputs, needed for d gate
+                ent += [(2, "y_attn", (M, D), BF), (2, "y_mlp", (M, D), BF)]
+            return ent
         # single blocks keep cat[attn | gelu(mlp)] — the input of proj_out — in ONE [M, 5D] buffer: attention and the GELU epilogue
         # write straight into its column ranges (no concat), proj_out is a plain K = 5D contraction, and the buffer is the LoRA
         # input of proj_out in the backward
-        ws["sgl"] = [dict(stats=e(2, M, dt=torch.float32), qkv=e(M, 3 * D), cat=e(M, 5 * D), lse=e(B, H, S, dt=torch.float32),
-                          u=e(M, 4 * D)) for _ in range(ns)]
+        ent = [(0, "stats", (2, M), f32), (0, "qkv", (M, 3 * D), BF), (0, "cat", (M, 5 * D), BF), (0, "lse", (B, H, S), f32),
+               (0, "u", (M, 4 * D), BF)]
+        if train and any(self._keeps_gate_out(l, "sgl") for l in blocks):
+            ent.append((1, "y_out", (M, D), BF))
+        return ent
+
+    def _fixed_entries(self, B, T, Limg, train, nblk, extra):
+        """([(name, shape, dtype)] allocated before the saved dicts, [...] after them): every workspace buffer whose size does
+        not depend on the activation plan.  `extra`: the family's conditioning buffers [(name, shape)] (bf16), allocated last."""
+        D, H, S, Mi, f32 = self.D, self.H, T + Limg, B * Limg, torch.float32
+        M = B * S
+        pre = [("X", (nblk + 1 if train else 2, M, D), BF), ("xm", (M, D), BF), ("h", (M, 4 * D), BF),
+               ("Q", (B, H, S, 128), BF), ("K", (B, H, S, 128), BF), ("V", (B, H, S, 128), BF)]
+        post = [("hn", (Mi, D), BF), ("pred", (Mi, self.C_out), BF), ("fstats", (2, Mi), f32)]
+        post += [(("loraT", key), (Mi if key[2] == 0 else B * T, site.n * PAD), BF) for key, site in self.sites.items()]
+        if train:
+            post += [("dX", (2, M, D), BF), ("dY", (M, D), BF), ("dbig", (M, 4 * D), BF), ("dqkv", (M, 3 * D), BF), ("dxm", (M, D), BF),
+                     ("dOj", (B, H, S, 128), BF), ("dK", (B, H, S, 128), BF), ("dV", (B, H, S, 128), BF), ("dQ", (B, H, S, 128), f32),
+                     ("delta", (B, H, S), f32), ("U", (M, 3 * PAD), BF), ("dhn", (Mi, D), BF), ("dpred", (Mi, self.C_out), BF),
+                     ("loss", (1,), f32)]
+        return pre, post + [(k, s, BF) for k, s in extra]
+
+    def _activation_limit_now(self):
+        if self._activation_limit is not None:
+            return self._activation_limit
+        if self.dev.type != "cuda":  # host-only models: nothing to plan against
+            return None
+        return torch.cuda.mem_get_info(self.dev)[0] - ACTIVATION_HEADROOM
+
+    def _alloc_common(self, ws, B, T, Limg, train, n_double, n_single=0, extra=()):
+        """The workspace of one (B, T, Limg, train) shape.  Training: every block either keeps its own saved dict or, when the
+        activation plan recomputes it, points at the one scratch dict of its kind (plan_activation_memory; planned before
+        anything is allocated)."""
+        D = self.D
+        Mt, Mi = B * T, B * Limg
+        M, S = Mt + Mi, T + Limg
+        nbytes = lambda shape, dt: math.prod(shape) * dt.itemsize
+        ws.update(B=B, T=T, Limg=Limg, S=S, Mt=Mt, Mi=Mi, M=M)
+        nblk = n_double + n_single
+        nd = n_double if train else min(1, n_double)
+        ns = n_single if train else min(1, n_single)
+        pre, post = self._fixed_entries(B, T, Limg, train, nblk, extra)
+        kinds = [("dbl", l) for l in range(nd)] + [("sgl", l) for l in range(ns)]
+        plan = ActivationPlan((), 0, 0, 0, None)
+        if train:
+            per_block = [(k, {n: nbytes(s, dt) for _, n, s, dt in self._saved_entries(k, (l,), B, S, True)}) for k, l in kinds]
+            plan = plan_activation_memory(per_block, sum(nbytes(s, dt) for _, s, dt in pre + post), self._activation_limit_now())
+        ws["plan"] = plan
+        for name, shape, dt in pre:
+            ws[name] = torch.empty(shape, device=self.dev, dtype=dt)
+        for kind, n in (("dbl", nd), ("sgl", ns)):
+            first = n_double if kind == "sgl" else 0  # global index of the kind's block 0
+            rec = [l for l in range(n) if first + l in plan.recompute]
+            slots = [([l], {}) for l in range(n) if first + l not in plan.recompute] + ([(rec, {})] if rec else [])
+            ents = [(d, self._saved_entries(kind, ls, B, S, train)) for ls, d in slots]
+            for g in (0, 1, 2):
+                for d, ent in ents:
+                    for grp, name, shape, dt in ent:
+                        if grp == g:
+                            d[name] = torch.empty(shape, device=self.dev, dtype=dt)
+            ws[kind] = [next(d for ls, d in slots if l in ls) for l in range(n)]
         for blk in ws["sgl"]:
             blk["O"], blk["h"] = blk["cat"][:, :D], blk["cat"][:, D:]
-        if train:
-            for l, blk in enumerate(ws["sgl"]):
-                if l in self.mod_sites.get("sgl", {}).get("rows", ()):
-                    blk["y_out"] = e(M, D)
-        ws["hn"], ws["pred"] = e(Mi, D), e(Mi, self.C_out)
-        ws["fstats"] = e(2, Mi, dt=torch.float32)
-        self._alloc_lora_T(ws)
-        if train:
-            ws["dX"] = e(2, M, D)
-            ws["dY"], ws["dbig"], ws["dqkv"], ws["dxm"] = e(M, D), e(M, 4 * D), e(M, 3 * D), e(M, D)
-            ws["dOj"], ws["dK"], ws["dV"] = e(B, H, S, 128), e(B, H, S, 128), e(B, H, S, 128)
-            ws["dQ"] = e(B, H, S, 128, dt=torch.float32)
-            ws["delta"] = e(B, H, S, dt=torch.float32)
-            ws["U"] = e(M, 3 * PAD)
-            ws["dhn"], ws["dpred"] = e(Mi, D), e(Mi, self.C_out)
-            ws["loss"] = torch.zeros(1, device=self.dev, dtype=torch.float32)
+        ws["loraT"] = {}
+        for name, shape, dt in post:
+            if isinstance(name, tuple):
+                ws["loraT"][name[1]] = torch.zeros(shape, device=self.dev, dtype=dt)
+            elif name == "loss":
+                ws["loss"] = torch.zeros(shape, device=self.dev, dtype=dt)
+            else:
+                ws[name] = torch.empty(shape, device=self.dev, dtype=dt)
         return ws
 
     def _get_workspace(self, key, build):

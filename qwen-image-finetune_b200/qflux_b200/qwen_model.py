@@ -10,8 +10,9 @@ launches and owns the HBM layout (see mmdit_base.py / DESIGN.md §3):
   * frozen weights live in layer-stacked fused tensors (q|k|v concatenated per stream, both streams adjacent) so one
     grouped wgmma GEMM serves the image and text stream of a block;
   * LoRA factors live zero-padded to 64 rows/cols so they enter the K loop of the base GEMM as one extra k-block;
-  * activations needed by the backward are kept in HBM (no recompute of GEMMs; on an 80 GB H100 they are what limits the batch):
-    block inputs, LayerNorm statistics, pre-norm q|k|v, attention output + logsumexp, mid residual, MLP pre-activation.
+  * activations needed by the backward are kept in HBM: block inputs, LayerNorm statistics, pre-norm q|k|v, attention output +
+    logsumexp, mid residual, MLP pre-activation.  On an 80 GB H100 they are what limits the batch, so the blocks whose saved
+    tensors do not fit keep only their input and are re-run right before their backward (`activation_plan`, DESIGN.md §3).
 
 No CPU path, no eager-PyTorch fallback: every op raises if the tensors are not on a CUDA device.
 """
@@ -126,15 +127,10 @@ class QwenImageB200(FusedMMDiTBase):
 
     # ------------------------------------------------------------------------------------------------ workspace
     def _workspace(self, B, T, Limg, train: bool):
-        def build():
-            ws = self._alloc_common({}, B, T, Limg, train, self.L)
-            e = lambda *s, dt=BF: torch.empty(*s, device=self.dev, dtype=dt)
-            ws["sin"], ws["t1"], ws["temb"] = e(B, 256), e(B, self.D), e(B, self.D)
-            ws["mods"] = e(B, self.L * 2 * 6 * self.D)
-            ws["fmod"] = e(B, 2 * self.D)
-            ws["txt_n"] = e(B * T, self.J)
-            return ws
-        return self._get_workspace((B, T, Limg, train), build)
+        D = self.D
+        extra = [("sin", (B, 256)), ("t1", (B, D)), ("temb", (B, D)), ("mods", (B, self.L * 2 * 6 * D)), ("fmod", (B, 2 * D)),
+                 ("txt_n", (B * T, self.J))]
+        return self._get_workspace((B, T, Limg, train), lambda: self._alloc_common({}, B, T, Limg, train, self.L, extra=extra))
 
     def _rope(self, img_shapes, T):
         key = (tuple(tuple(s) for s in img_shapes), T)
