@@ -209,6 +209,23 @@ int qfx_fused_adamw(const qfx_adamw_tensor* tensors, const int* chunks, int n_ch
                     float beta2, float eps, float weight_decay, int step, void* stream);
 
 /* ------------------------------------------------------------------------------------------------------------------
+ * NF4 frozen weights (4-bit base checkpoints: bitsandbytes `Linear4bit`, whose forward dequantizes the weight to bf16 and runs a
+ * plain matmul, bitsandbytes/functional.py dequantize_4bit).  One launch dequantizes up to QFX_NF4_MAX_SEGMENTS tensors (the NF4
+ * matrices of one block) into bf16:  out[i] = bf16_rn(NF4[nibble_i] * absmax[i / blocksize])  with the product in fp32,
+ * element 2k = high nibble of codes[k], NF4 = bitsandbytes' built-in code book.  absmax is fp32, one value per `blocksize` elements
+ * (nested absmax is folded by the caller).  n % 32 == 0, blocksize % 32 == 0 and divides n; codes and out 16-byte aligned.
+ * The segment table is read on the host and passed by value: no device table, no host synchronisation. */
+#define QFX_NF4_MAX_SEGMENTS 8
+typedef struct {
+  const void* codes;    /* n / 2 bytes */
+  const float* absmax;  /* n / blocksize */
+  void* out;            /* n bf16 */
+  int64_t n;
+  int blocksize;
+} qfx_nf4_segment;
+int qfx_nf4_dequant(const qfx_nf4_segment* segs, int nseg, void* stream);
+
+/* ------------------------------------------------------------------------------------------------------------------
  * Peer memory for sharded frozen weights (replaces FSDP's per-module all-gather, base_trainer.py:333-382, for the frozen block
  * weights).  A rank's weight shard lives in an allocation made by qfx_peer_alloc; its 64-byte handle is sent to the other ranks
  * of the node (any host transport), which map it with qfx_peer_open.  qfx_peer_copy_async then pulls bytes from a mapped peer

@@ -65,10 +65,13 @@ class FluxB200(FusedMMDiTBase):
     }
     _ADALN = ("norm1.linear", "norm1_context.linear")
     _PER_SINGLE = ("s_mod_w", "s_mod_b", "s_qkv_w", "s_qkv_b", "s_mlp_w", "s_mlp_b", "s_out_w", "s_out_b", "s_qknorm_w")
+    _NF4_KINDS = FusedMMDiTBase._NF4_KINDS + ("s_mod_w", "s_qkv_w", "s_mlp_w", "s_out_w")
+    _SINGLE_MATS = {**{nm: grp + "_w" for nm, (grp, _) in _SINGLE_LINEARS.items()}, "norm.linear": "s_mod_w"}
 
-    def __init__(self, cfg: FluxB200Config, device="cuda", _host_only: bool = False):
+    def __init__(self, cfg: FluxB200Config, device="cuda", _host_only: bool = False, frozen_weights="bf16", nf4_blocksize: int = 64):
+        """frozen_weights / nf4_blocksize: as for QwenImageB200 (4-bit base checkpoints)."""
         super().__init__()
-        self._init_common(device, _host_only)
+        self._init_common(device, _host_only, frozen_weights, nf4_blocksize)
         assert cfg.attention_head_dim == 128, "the sm_90a attention kernels are specialised for head_dim 128"
         self.config = cfg
         D = cfg.num_attention_heads * cfg.attention_head_dim
@@ -79,25 +82,27 @@ class FluxB200(FusedMMDiTBase):
         self.Pp = cfg.pooled_projection_dim
         L, Ls, J = self.L, self.Ls, self.J
         z = lambda *s: torch.zeros(*s, device=self.dev, dtype=BF)
+        f = self._frozen
         self.w = {
             "x_in_w": z(D, self.C_in), "x_in_b": z(D), "ctx_in_w": z(D, J), "ctx_in_b": z(D),
             "t1_w": z(D, 256), "t1_b": z(D), "t2_w": z(D, D), "t2_b": z(D),
             "g1_w": z(D, 256), "g1_b": z(D), "g2_w": z(D, D), "g2_b": z(D),
             "p1_w": z(D, self.Pp), "p1_b": z(D), "p2_w": z(D, D), "p2_b": z(D),
-            "mod_w": z(L, 2, 6 * D, D), "mod_b": z(L, 2, 6 * D),
-            "qkv_w": z(L, 2, 3 * D, D), "qkv_b": z(L, 2, 3 * D),
-            "out_w": z(L, 2, D, D), "out_b": z(L, 2, D),
-            "up_w": z(L, 2, 4 * D, D), "up_b": z(L, 2, 4 * D),
-            "down_w": z(L, 2, D, 4 * D), "down_b": z(L, 2, D),
+            "mod_w": f("mod_w", L, 2, 6 * D, D), "mod_b": z(L, 2, 6 * D),
+            "qkv_w": f("qkv_w", L, 2, 3 * D, D), "qkv_b": z(L, 2, 3 * D),
+            "out_w": f("out_w", L, 2, D, D), "out_b": z(L, 2, D),
+            "up_w": f("up_w", L, 2, 4 * D, D), "up_b": z(L, 2, 4 * D),
+            "down_w": f("down_w", L, 2, D, 4 * D), "down_b": z(L, 2, D),
             "qknorm_w": torch.ones(L, 4, 128, device=self.dev, dtype=BF),
-            "s_mod_w": z(Ls, 3 * D, D), "s_mod_b": z(Ls, 3 * D),
-            "s_qkv_w": z(Ls, 3 * D, D), "s_qkv_b": z(Ls, 3 * D),
-            "s_mlp_w": z(Ls, 4 * D, D), "s_mlp_b": z(Ls, 4 * D),
-            "s_out_w": z(Ls, D, 5 * D), "s_out_b": z(Ls, D),
+            "s_mod_w": f("s_mod_w", Ls, 3 * D, D), "s_mod_b": z(Ls, 3 * D),
+            "s_qkv_w": f("s_qkv_w", Ls, 3 * D, D), "s_qkv_b": z(Ls, 3 * D),
+            "s_mlp_w": f("s_mlp_w", Ls, 4 * D, D), "s_mlp_b": z(Ls, 4 * D),
+            "s_out_w": f("s_out_w", Ls, D, 5 * D), "s_out_b": z(Ls, D),
             "s_qknorm_w": torch.ones(Ls, 2, 128, device=self.dev, dtype=BF),
             "norm_out_w": z(2 * D, D), "norm_out_b": z(2 * D),
             "proj_out_w": z(self.C_out, D), "proj_out_b": z(self.C_out),
         }
+        self._finish_frozen()
 
     def _wb(self, l, grp, s):
         if l < 0:
@@ -107,8 +112,8 @@ class FluxB200(FusedMMDiTBase):
         return self.w[grp + "_w"][l, s], self.w[grp + "_b"][l, s]
 
     # ------------------------------------------------------------------------------------------------ names
-    def _weight_views(self) -> dict:
-        w, D, out = self.w, self.D, {}
+    def _weight_views(self, store: bool = False) -> dict:
+        (w, blocks), D, out = self._view_source(store), self.D, {}
         out["x_embedder.weight"], out["x_embedder.bias"] = w["x_in_w"], w["x_in_b"]
         out["context_embedder.weight"], out["context_embedder.bias"] = w["ctx_in_w"], w["ctx_in_b"]
         for pre, nm in (("t", "timestep_embedder"), ("p", "text_embedder")) + ((("g", "guidance_embedder"),) if self.config.guidance_embeds else ()):
@@ -117,8 +122,8 @@ class FluxB200(FusedMMDiTBase):
             out[p + "linear_2.weight"], out[p + "linear_2.bias"] = w[pre + "2_w"], w[pre + "2_b"]
         out["norm_out.linear.weight"], out["norm_out.linear.bias"] = w["norm_out_w"], w["norm_out_b"]
         out["proj_out.weight"], out["proj_out.bias"] = w["proj_out_w"], w["proj_out_b"]
-        self._double_weight_views(out)
-        for l in range(self.Ls if self._sharded is None else 0):
+        self._double_weight_views(out, w, blocks)
+        for l in range(self.Ls if blocks else 0):
             b = f"single_transformer_blocks.{l}."
             out[b + "norm.linear.weight"], out[b + "norm.linear.bias"] = w["s_mod_w"][l], w["s_mod_b"][l]
             out[b + "attn.norm_q.weight"], out[b + "attn.norm_k.weight"] = w["s_qknorm_w"][l, 0], w["s_qknorm_w"][l, 1]
@@ -251,7 +256,7 @@ class FluxB200(FusedMMDiTBase):
             lib.add_bf16(ws["temb"], ws["gemb"], ws["temb"])
         self._mlp2(pooled_projections.to(BF).contiguous(), "p", ws["pemb"], ws["e1"])
         lib.add_bf16(ws["temb"], ws["pemb"], ws["temb"])
-        if self._sharded is None:  # all modulation linears of a kind in one launch; sharded weights produce them block by block
+        if self._blk_rings is None:  # all modulation linears of a kind in one launch; ringed weights produce them block by block
             lib.gemv_act(ws["temb"], w["mod_w"].view(L * 2 * 6 * D, D), w["mod_b"].view(-1), ws["mods"], act=1)
             if Ls:
                 lib.gemv_act(ws["temb"], w["s_mod_w"].view(Ls * 3 * D, D), w["s_mod_b"].view(-1), ws["smods"], act=1)

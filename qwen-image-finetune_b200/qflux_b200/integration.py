@@ -26,7 +26,9 @@ def _cfg_get(cfg, k, default=None):
 def from_reference(ref_model, device=None, _host_only: bool = False):
     """Build the fused model for a loaded reference / diffusers transformer (`QwenImageTransformer2DModel` or
     `FluxTransformer2DModel`): same config, weights copied through the shared state-dict key names, and — when the module already
-    carries a PEFT adapter (`peft_config`) — the same adapter with the same factors."""
+    carries a PEFT adapter (`peft_config`) — the same adapter with the same factors.  A 4-bit base model (bitsandbytes `Linear4bit`,
+    NF4) gives a model whose block matrices stay NF4-resident (`frozen_weights`, picked per stacked kind from what the state dict holds)."""
+    from . import nf4
     from .flux_model import FluxB200, FluxB200Config
     from .qwen_model import QwenB200Config, QwenImageB200
     cfg = ref_model.config
@@ -36,13 +38,30 @@ def from_reference(ref_model, device=None, _host_only: bool = False):
     C, M = (FluxB200Config, FluxB200) if is_flux else (QwenB200Config, QwenImageB200)
     kw = {k: _cfg_get(cfg, k) for k in C.__dataclass_fields__ if _cfg_get(cfg, k) is not None}
     kw["axes_dims_rope"] = tuple(kw.get("axes_dims_rope", (16, 56, 56)))
-    dit = M(C(**kw), device=device, _host_only=_host_only)
     sd = ref_model.state_dict()
+    plain, quant = nf4.split_state_dict(sd)
+    nf4_kw = {}
+    if quant:
+        kinds, sizes = {}, set()
+        for k, q in quant.items():
+            kk = k.replace(".base_layer.", ".")
+            kind = M._matrix_kind(kk[len("transformer."):] if kk.startswith("transformer.") else kk)
+            if kind is not None:
+                kinds[kind] = k
+                sizes.add(q.blocksize)
+        if len(sizes) > 1:
+            raise nf4.QfxError(f"the NF4 block matrices use blocksizes {sorted(sizes)}; the fused layout takes one per model")
+        if kinds:
+            nf4_kw = dict(frozen_weights=tuple(kinds), nf4_blocksize=sizes.pop())
+    dit = M(C(**kw), device=device, _host_only=_host_only, **nf4_kw)
     peft_cfg = getattr(ref_model, "peft_config", None)
     if peft_cfg:
         (name, pc), = list(peft_cfg.items())
         dit.add_adapter(pc, adapter_name=name)
-    dit.load_state_dict(sd, strict=True)
+    if quant or dit.frozen_weights != "bf16":
+        dit._load_nf4(plain, quant, strict=True)
+    else:
+        dit.load_state_dict(sd, strict=True)
     return dit
 
 

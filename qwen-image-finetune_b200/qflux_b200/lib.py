@@ -439,6 +439,28 @@ def attn_fwd(Q, K, V, out_txt, out_img, split, lse=None, kv_len=None, scale=None
                     ptr(lse), ptr(kv_len), ptr(txt_len), B, H, S, scale, cur_stream()), "qfx_attn_fwd")
 
 
+# ---------------------------------------------------------------------------------------------------- NF4 frozen weights (nf4.py)
+class Nf4Segment(C.Structure):
+    _fields_ = [("codes", C.c_void_p), ("absmax", C.c_void_p), ("out", C.c_void_p), ("n", C.c_int64), ("blocksize", C.c_int)]
+
+
+NF4_MAX_SEGMENTS = 8
+_nf4 = _sig("qfx_nf4_dequant", C.POINTER(Nf4Segment), _i, _vp)
+
+
+def nf4_dequant(segments):
+    """segments: [(codes uint8 [n/2], absmax fp32 [n/blocksize], out bf16 [n], blocksize)], contiguous; ONE launch fills every out."""
+    arr = (Nf4Segment * len(segments))()
+    for i, (codes, absmax, out, bs) in enumerate(segments):
+        require_cuda(codes, absmax, out)
+        n = out.numel()
+        assert codes.dtype == torch.uint8 and absmax.dtype == torch.float32 and out.dtype == torch.bfloat16
+        assert codes.is_contiguous() and absmax.is_contiguous() and out.is_contiguous()
+        assert codes.numel() * 2 == n and absmax.numel() * bs == n
+        arr[i] = Nf4Segment(codes.data_ptr(), absmax.data_ptr(), out.data_ptr(), n, bs)
+    check(_nf4(arr, len(segments), cur_stream()), "qfx_nf4_dequant")
+
+
 # ---------------------------------------------------------------------------------------------------- peer memory (sharding.py)
 PEER_HANDLE_BYTES = 64
 for _f in ("qfx_peer_alloc", "qfx_peer_free", "qfx_peer_open", "qfx_peer_close", "qfx_peer_copy_async"):

@@ -111,15 +111,18 @@ class FusedMMDiTBase(nn.Module):
     _ADALN = ("", "")           # sub-module names of a double block's (image, text) AdaLN modulation Linears
     _PER_LAYER = ("mod_w", "mod_b", "qkv_w", "qkv_b", "out_w", "out_b", "up_w", "up_b", "down_w", "down_b", "qknorm_w")
     _PER_SINGLE = ()
+    _NF4_KINDS = ("mod_w", "qkv_w", "out_w", "up_w", "down_w")  # the stacked matrices a 4-bit base checkpoint keeps NF4-resident
+    _SINGLE_MATS: dict = {}     # sub-module name of a single-block Linear -> its stacked kind (FLUX)
     _sharded_s = None           # sharding.ShardedBlocks of the single blocks once shard_frozen_weights() has run
 
     def _weight_views(self) -> dict:
         raise NotImplementedError
 
-    def _double_weight_views(self, out: dict) -> dict:
-        """Adds the state-dict entries of every double block to `out` (sharded block weights are not addressable as full tensors)."""
-        w, D = self.w, self.D
-        for l in range(self.L if self._sharded is None else 0):
+    def _double_weight_views(self, out: dict, w: dict, blocks: bool) -> dict:
+        """Adds the state-dict entries of every double block of `w` to `out` when `blocks` (block weights that come through a ring
+        are not addressable as full tensors)."""
+        D = self.D
+        for l in range(self.L if blocks else 0):
             b = f"transformer_blocks.{l}."
             for s, nm in enumerate(self._ADALN):
                 out[b + nm + ".weight"], out[b + nm + ".bias"] = w["mod_w"][l, s], w["mod_b"][l, s]
@@ -161,10 +164,42 @@ class FusedMMDiTBase(nn.Module):
             return self.w[grp + "_w"], self.w[grp + "_b"]
         return self.w[grp + "_w"][l, s], self.w[grp + "_b"][l, s]
 
+    def _view_source(self, store: bool):
+        """(weights dict, whether block entries are included) for `_weight_views`.  store=True: every block, with the NF4-resident
+        kinds as meta tensors of their bf16 shape — their views' storage offsets address the codes and absmax (load_state_dict)."""
+        if not store:
+            return self.w, self._blk_rings is None
+        w = dict(self.w)
+        for k, (codes, _) in self._nf4_store.items():
+            w[k] = torch.empty(*codes.shape[:-1], codes.shape[-1] * 2, device="meta", dtype=BF)
+        return w, True
+
+    @classmethod
+    def _matrix_kind(cls, key: str):
+        """Stacked kind ("qkv_w", "s_mod_w", ...) of the block Linear whose weight is `key` (None: not a block matrix)."""
+        m = re.fullmatch(r"(single_)?transformer_blocks\.\d+\.(.+)\.weight", key)
+        if m is None:
+            return None
+        if m.group(1):
+            return cls._SINGLE_MATS.get(m.group(2))
+        if m.group(2) in cls._ADALN:
+            return "mod_w"
+        grp = cls._DOUBLE_LINEARS.get(m.group(2))
+        return None if grp is None else grp[0] + "_w"
+
     # -----------------------------------------------------------------------------------------------------------------
-    def _init_common(self, device, host_only):
+    def _init_common(self, device, host_only, frozen_weights="bf16", nf4_blocksize=64):
+        """frozen_weights: "bf16" (block weights resident in bf16), "nf4" (every stacked block matrix NF4-resident: a 4-bit base
+        checkpoint) or the set of stacked kinds that are (`from_reference` picks what the checkpoint holds)."""
         if not host_only and not torch.cuda.is_available():
             raise lib.QfxError(f"{type(self).__name__} needs a CUDA device (sm_90a); there is no CPU fallback")
+        kinds = () if frozen_weights == "bf16" else self._NF4_KINDS if frozen_weights == "nf4" else tuple(frozen_weights)
+        if isinstance(frozen_weights, str) and frozen_weights not in ("bf16", "nf4") or not set(kinds) <= set(self._NF4_KINDS):
+            raise lib.QfxError(f"frozen_weights={frozen_weights!r}: 'bf16', 'nf4' or a subset of {self._NF4_KINDS}")
+        self._nf4_kinds, self.nf4_blocksize = tuple(k for k in self._NF4_KINDS if k in kinds), int(nf4_blocksize)
+        self._nf4_store = {}     # NF4-resident kind -> (codes uint8 [L, ..., in/2], absmax fp32 [L, n/blocksize])
+        self._nf4_rings = None   # sharding.Nf4Blocks of (double, single) blocks
+        self._blk_rings = None   # (double, single) rings the block weights come through: NF4 dequantization or sharding
         self.dev = torch.device(device)
         self.sites = {}          # (l, grp, s) -> LoraSite   (l = -1: input embedders)
         self.mod_sites = {}      # kind -> dict(idx=[row indices], names=[...], A=[n, r, D], B=[n, C, r], ga, gb)  (AdaLN linears)
@@ -177,10 +212,41 @@ class FusedMMDiTBase(nn.Module):
         self._rope_cache = {}
         self.gradient_checkpointing = False  # accepted for interface compatibility (see enable_gradient_checkpointing)
         self._activation_limit = None  # bytes the training workspace may take; None: free device memory - ACTIVATION_HEADROOM
-        self._sharded = None     # sharding.ShardedBlocks once shard_frozen_weights() has run
+        self._sharded = None     # sharding.ShardedBlocks once shard_frozen_weights() has run (weights sharded across ranks)
         self._bands_cache = {}   # (valid image rows per sample, Limg) -> lib.RowBands (ragged GEMM row bands)
         self._infer_graphs, self.use_cuda_graph_inference = GraphCache(8, "the inference forward"), True  # see _infer
         self._fwd_gen = 0        # bumped by every forward: autograd nodes of an older forward refuse to run (their activations are gone)
+
+    def _frozen(self, kind, *shape):
+        """A stacked block matrix [L, ..., out, in]: bf16 zeros, or — NF4-resident — its codes and absmax (in `self._nf4_store`; the
+        bf16 stack is never allocated and `self.w[kind]` becomes a ring view in `_finish_frozen`)."""
+        if kind not in self._nf4_kinds:
+            return torch.zeros(*shape, device=self.dev, dtype=BF)
+        if shape[-1] % self.nf4_blocksize:
+            raise lib.QfxError(f"{kind}: NF4 blocksize {self.nf4_blocksize} does not divide in_features {shape[-1]}")
+        n = math.prod(shape[1:])
+        self._nf4_store[kind] = (torch.zeros(*shape[:-1], shape[-1] // 2, device=self.dev, dtype=torch.uint8),
+                                 torch.zeros(shape[0], n // self.nf4_blocksize, device=self.dev, dtype=torch.float32))
+        return None
+
+    def _finish_frozen(self):
+        """NF4-resident kinds: one two-slot ring per block kind, filled by dequantizing a block right before it runs."""
+        if not self._nf4_kinds:
+            return
+        from .sharding import Nf4Blocks
+        rings = []
+        for per, n in ((self._PER_LAYER, self.L), (self._PER_SINGLE, self.Ls)):
+            st = {k: (*self._nf4_store[k], tuple(self._nf4_store[k][0].shape[1:-1]) + (self._nf4_store[k][0].shape[-1] * 2,))
+                  for k in per if k in self._nf4_store}
+            rings.append(Nf4Blocks(st, n, self.nf4_blocksize) if st else None)
+            for k in st:
+                self.w[k] = rings[-1].rings[k]
+        self._nf4_rings = self._blk_rings = tuple(rings)
+
+    @property
+    def frozen_weights(self) -> str:
+        """How the frozen block weights are stored: "bf16", or "nf4" (NF4-resident, dequantized block by block)."""
+        return "nf4" if self._nf4_kinds else "bf16"
 
     @property
     def device(self):
@@ -199,6 +265,9 @@ class FusedMMDiTBase(nn.Module):
         from .sharding import ShardedBlocks
         if self._sharded is not None:
             return self
+        if self._nf4_kinds:
+            raise lib.QfxError("shard_frozen_weights: the frozen weights are NF4-resident (frozen_weights='nf4'); sharded NF4 is not "
+                               "supported — shard a bf16 model or train the NF4 model on one GPU per replica")
         self._sharded = ShardedBlocks({k: self.w[k] for k in self._PER_LAYER}, self.L, group, gather=gather)
         for k in self._PER_LAYER:
             self.w[k] = self._sharded.rings[k]
@@ -206,28 +275,37 @@ class FusedMMDiTBase(nn.Module):
             self._sharded_s = ShardedBlocks({k: self.w[k] for k in self._PER_SINGLE}, self.Ls, group, gather=gather)
             for k in self._PER_SINGLE:
                 self.w[k] = self._sharded_s.rings[k]
+        self._blk_rings = (self._sharded, self._sharded_s)
         if torch.cuda.is_available():
             torch.cuda.empty_cache()
         return self
 
     def _ring(self, blk):
-        """(ring, local index) of global block `blk` (double blocks first, then single blocks)."""
-        return (self._sharded, blk) if blk < self.L else (self._sharded_s, blk - self.L)
+        """(ring or None, local index) of global block `blk` (double blocks first, then single blocks)."""
+        return (self._blk_rings[0], blk) if blk < self.L else (self._blk_rings[1], blk - self.L)
 
     def _acquire(self, blk, nxt):
-        """Sharded weights: make block `blk` resident and start fetching block `nxt` (if there is one)."""
+        """Ringed weights: make block `blk` resident and start filling block `nxt` (if there is one)."""
         ring, l = self._ring(blk)
-        ring.acquire(l)
+        if ring is not None:
+            ring.acquire(l)
         if 0 <= nxt < self.L + self.Ls:
             r2, l2 = self._ring(nxt)
-            r2.prefetch(l2)
+            if r2 is not None:
+                r2.prefetch(l2)
 
     def _release(self, blk):
         ring, l = self._ring(blk)
-        ring.release(l)
+        if ring is not None:
+            ring.release(l)
+
+    def _join_nf4_rings(self):
+        for ring in self._nf4_rings or ():
+            if ring is not None:
+                ring.join()
 
     def _block_mods(self, ws, blk):
-        """Sharded weights: the base modulation vectors of block `blk` (plus their LoRA), from its now resident weights."""
+        """Ringed weights: the base modulation vectors of block `blk` (plus their LoRA), from its now resident weights."""
         D, w = self.D, self.w
         if blk < self.L:
             lib.gemv_act(ws["temb"], w["mod_w"][blk].view(2 * 6 * D, D), w["mod_b"][blk].view(-1),
@@ -289,6 +367,13 @@ class FusedMMDiTBase(nn.Module):
 
     @torch.no_grad()
     def load_state_dict(self, sd, strict=True, assign=False):
+        """bf16 checkpoints, and 4-bit NF4 base checkpoints (bitsandbytes `Linear4bit` entries, nf4.py): NF4 block matrices go to the
+        NF4-resident storage of a model constructed with frozen_weights='nf4' (`from_reference` does), NF4 tensors outside the blocks
+        are dequantized to bf16 here."""
+        from . import nf4
+        plain, quant = nf4.split_state_dict(sd)
+        if quant or self._nf4_kinds:
+            return self._load_nf4(plain, quant, strict)
         views = self._weight_views()
         unexpected, seen = [], set()
         for k, v in sd.items():
@@ -302,6 +387,59 @@ class FusedMMDiTBase(nn.Module):
                 seen.add(lk)
             else:
                 unexpected.append(k)
+        missing = [k for k in list(views) + list(self._lora_params) if k not in seen]
+        if strict and (unexpected or [m for m in missing if "lora" not in m]):
+            raise KeyError(f"load_state_dict: missing {missing[:5]}..., unexpected {unexpected[:5]}...")
+        return missing, unexpected
+
+    def _load_nf4(self, plain, quant, strict):
+        """load_state_dict of a checkpoint with NF4 entries or into an NF4-resident model: every block entry is addressable here
+        (meta views stand for the NF4 kinds; a view's storage offset locates its rows in the codes / absmax stacks)."""
+        from . import nf4
+        views = self._weight_views(store=True)
+        unexpected, seen = [], set()
+
+        def canon(k):
+            k = k.replace(".base_layer.", ".")
+            return k[len("transformer."):] if k.startswith("transformer.") and k[len("transformer."):] in views else k
+
+        for k, v in plain.items():
+            kk, lk = canon(k), self._canonical_lora_key(k)
+            if kk in views:
+                if views[kk].is_meta:
+                    raise lib.QfxError(f"`{kk}` arrives in bf16, but {self._matrix_kind(kk)} is NF4-resident in this model "
+                                       f"(frozen_weights={self._nf4_kinds!r}): the layers of a stacked kind must arrive in one format; "
+                                       f"construct with frozen_weights='bf16' for a bf16 checkpoint")
+                views[kk].copy_(v.to(self.dev, BF))
+                seen.add(kk)
+            elif lk in self._lora_params:
+                self._lora_params[lk].copy_(v.to(self.dev, BF))
+                seen.add(lk)
+            else:
+                unexpected.append(k)
+        for k, q in quant.items():
+            kk = canon(k)
+            if kk not in views:
+                unexpected.append(k)
+                continue
+            t = views[kk]
+            if tuple(t.shape) != q.shape:
+                raise lib.QfxError(f"`{kk}`: NF4 shape {q.shape}, the model expects {tuple(t.shape)}")
+            if not t.is_meta:
+                if self._matrix_kind(kk) is not None:
+                    raise lib.QfxError(f"`{kk}` is NF4 but this model keeps {self._matrix_kind(kk)} in bf16 (frozen_weights="
+                                       f"{'bf16' if not self._nf4_kinds else self._nf4_kinds!r}): construct it with frozen_weights='nf4' "
+                                       f"(from_reference does) for a 4-bit base checkpoint")
+                t.copy_(nf4.dequantize(q).to(self.dev))  # outside the blocks: bf16 in the existing layout
+            else:
+                if q.blocksize != self.nf4_blocksize:
+                    raise lib.QfxError(f"`{kk}`: NF4 blocksize {q.blocksize}, the model was constructed with nf4_blocksize="
+                                       f"{self.nf4_blocksize}")
+                codes, absmax = self._nf4_store[self._matrix_kind(kk)]
+                o, n = t.storage_offset(), t.numel()
+                codes.view(-1)[o // 2:(o + n) // 2].copy_(q.codes.to(self.dev))
+                absmax.view(-1)[o // q.blocksize:(o + n) // q.blocksize].copy_(q.absmax.to(self.dev))
+            seen.add(kk)
         missing = [k for k in list(views) + list(self._lora_params) if k not in seen]
         if strict and (unexpected or [m for m in missing if "lora" not in m]):
             raise KeyError(f"load_state_dict: missing {missing[:5]}..., unexpected {unexpected[:5]}...")
@@ -481,6 +619,8 @@ class FusedMMDiTBase(nn.Module):
         term, so a merged adapter is represented by lora_B = 0); the bf16 rounding of W + delta is PEFT's own."""
         if self._sharded is not None:
             raise lib.QfxError("merge_adapter: the frozen weights are sharded; merge on a replicated model")
+        if self._nf4_kinds:
+            raise lib.QfxError("merge_adapter: the frozen weights are NF4-resident (frozen_weights='nf4'); merge on a bf16 model")
         if not self._lora_params or getattr(self, "_merged", None):
             return
         views, parked = self._weight_views(), {}
@@ -585,8 +725,12 @@ class FusedMMDiTBase(nn.Module):
                     continue
             if len(sel) == len(ms["names"]):  # everything (the un-sharded path): no list indexing -> no host-to-device index upload, which
                 A, Bm, idx = ms["A"], ms["B"], ms["idx"]  # would be illegal inside the CUDA-graph capture of the step
-            else:
-                A, Bm, idx = ms["A"][sel], ms["B"][sel], ms["idx"][sel]
+            else:  # one block's rows (ringed weights): a device index made once per block, on the eager first step, so capture uploads nothing
+                cache = ms.setdefault("sel_dev", {})
+                if tuple(sel) not in cache:
+                    cache[tuple(sel)] = torch.tensor(sel, device=self.dev)
+                sel_t = cache[tuple(sel)]
+                A, Bm, idx = ms["A"].index_select(0, sel_t), ms["B"].index_select(0, sel_t), ms["idx"].index_select(0, sel_t)
             t = torch.matmul(x.float()[None], A.float().transpose(1, 2)).to(BF)               # [n, B, r]
             d = torch.bmm(t.float(), Bm.float().transpose(1, 2)).to(BF)                       # [n, B, C]
             d = (d.float() * self.lora_scaling).to(BF)
@@ -598,7 +742,7 @@ class FusedMMDiTBase(nn.Module):
             if len(sel) == len(ms["names"]):
                 ws[key].copy_(t)
             else:
-                ws[key][sel] = t
+                ws[key].index_copy_(0, sel_t, t)
 
     def _mod_grad_buffers(self, ws):
         """fp32 accumulators for d mods (same layout as the modulation vectors), zeroed at the start of every backward."""
@@ -987,11 +1131,14 @@ class FusedMMDiTBase(nn.Module):
     def _blocks_and_head_fwd(self, ws, train):
         """Every block (double blocks, then single blocks) from the embedded tokens in ws["X"][0], then the output head on the image
         rows: AdaLayerNormContinuous (scale, shift) + proj_out.  Returns the prediction [B, Limg, C_out] (workspace memory)."""
-        D, L, Mt, w, sh = self.D, self.L, ws["Mt"], self.w, self._sharded
+        D, L, Mt, w, sh = self.D, self.L, ws["Mt"], self.w, self._blk_rings
         nb = L + self.Ls
         xi = lambda i: ws["X"][i] if train else ws["X"][i & 1]
+        for ring in self._nf4_rings or ():  # every forward fills the same blocks: eager, captured and replayed alike
+            if ring is not None:
+                ring.reset()
         for blk in range(nb):
-            if sh is not None:  # block blk's weights arrive by all-gather (block blk+1's gather starts now, on the side stream)
+            if sh is not None:  # block blk's weights arrive through its ring (block blk+1's fill starts now, on the side stream)
                 self._acquire(blk, blk + 1)
                 self._block_mods(ws, blk)
             if blk < L:
@@ -1000,6 +1147,7 @@ class FusedMMDiTBase(nn.Module):
                 self._single_fwd(ws, blk - L, xi(blk), xi(blk + 1), ws["sgl"][(blk - L) if train else 0])
             if sh is not None:
                 self._release(blk)
+        self._join_nf4_rings()
         Xl = ws["Xlast"] = xi(nb)
         lib.ln_modulate_fwd(Xl[Mt:], ws["hn"], ws["fmod"][:, D:], ws["fmod"][:, :D], ws["Limg"], ws["fstats"][0], ws["fstats"][1])
         lib.gemm([lib.gemm_problem(ws["hn"], w["proj_out_w"], ws["pred"], bias=w["proj_out_b"])], self.C_out, D)
@@ -1023,7 +1171,7 @@ class FusedMMDiTBase(nn.Module):
         for blk in range(nb - 1, -1, -1):
             dXn = ws["dX"][blk & 1]
             prev = self._last_gate(ws, blk - 1) if blk > 0 else None
-            if self._sharded is not None:
+            if self._blk_rings is not None:
                 self._acquire(blk, blk - 1)
             if blk in ws["plan"].recompute:  # regenerate the block's saved tensors into the scratch dict (its weights are resident now)
                 if blk < L:
@@ -1034,9 +1182,10 @@ class FusedMMDiTBase(nn.Module):
                 self._double_bwd(ws, blk, ws["X"][blk], dX, dXn, ws["dbl"][blk], self._mods(ws, blk), prev)
             else:
                 self._single_bwd(ws, blk - L, ws["X"][blk], dX, dXn, ws["sgl"][blk - L], prev)
-            if self._sharded is not None:
+            if self._blk_rings is not None:
                 self._release(blk)
             dX = dXn
+        self._join_nf4_rings()
         self._mod_lora_bwd(ws)
         for key, s, _ in self._embed_table().values():
             self._embed_bwd(ws, key, s, dX)

@@ -77,11 +77,12 @@ class QwenImageB200(FusedMMDiTBase):
     }
     _ADALN = ("img_mod.1", "txt_mod.1")
 
-    def __init__(self, cfg: QwenB200Config, device="cuda", _host_only: bool = False):
+    def __init__(self, cfg: QwenB200Config, device="cuda", _host_only: bool = False, frozen_weights="bf16", nf4_blocksize: int = 64):
         """`_host_only=True` (tests of the naming / LoRA-registry logic) allocates on `device` without requiring CUDA;
-        every compute entry point still raises on non-CUDA tensors."""
+        every compute entry point still raises on non-CUDA tensors.  frozen_weights="nf4": the block matrices of a 4-bit base
+        checkpoint stay NF4-resident (codes + fp32 absmax per `nf4_blocksize` elements) and are dequantized block by block."""
         super().__init__()
-        self._init_common(device, _host_only)
+        self._init_common(device, _host_only, frozen_weights, nf4_blocksize)
         assert cfg.attention_head_dim == 128, "the sm_90a attention kernels are specialised for head_dim 128"
         self.config = cfg
         # Multi-resolution batches with PADDED TEXT: "aligned" rotates a sample's image tokens where they sit ([T, T + L_b)), which makes
@@ -94,24 +95,26 @@ class QwenImageB200(FusedMMDiTBase):
         self.C_in, self.C_out = cfg.in_channels, cfg.patch_size ** 2 * cfg.out_channels
         L, J = self.L, self.J
         z = lambda *s: torch.zeros(*s, device=self.dev, dtype=BF)
+        f = self._frozen
         # frozen weights (plain tensors, not Parameters: they never receive gradients on this path)
         self.w = {
             "img_in_w": z(D, self.C_in), "img_in_b": z(D), "txt_norm_w": torch.ones(J, device=self.dev, dtype=BF),
             "txt_in_w": z(D, J), "txt_in_b": z(D),
             "t1_w": z(D, 256), "t1_b": z(D), "t2_w": z(D, D), "t2_b": z(D),
-            "mod_w": z(L, 2, 6 * D, D), "mod_b": z(L, 2, 6 * D),
-            "qkv_w": z(L, 2, 3 * D, D), "qkv_b": z(L, 2, 3 * D),
-            "out_w": z(L, 2, D, D), "out_b": z(L, 2, D),
-            "up_w": z(L, 2, 4 * D, D), "up_b": z(L, 2, 4 * D),
-            "down_w": z(L, 2, D, 4 * D), "down_b": z(L, 2, D),
+            "mod_w": f("mod_w", L, 2, 6 * D, D), "mod_b": z(L, 2, 6 * D),
+            "qkv_w": f("qkv_w", L, 2, 3 * D, D), "qkv_b": z(L, 2, 3 * D),
+            "out_w": f("out_w", L, 2, D, D), "out_b": z(L, 2, D),
+            "up_w": f("up_w", L, 2, 4 * D, D), "up_b": z(L, 2, 4 * D),
+            "down_w": f("down_w", L, 2, D, 4 * D), "down_b": z(L, 2, D),
             "qknorm_w": torch.ones(L, 4, 128, device=self.dev, dtype=BF),
             "norm_out_w": z(2 * D, D), "norm_out_b": z(2 * D),
             "proj_out_w": z(self.C_out, D), "proj_out_b": z(self.C_out),
         }
+        self._finish_frozen()
 
     # ------------------------------------------------------------------------------------------------ names
-    def _weight_views(self) -> dict:
-        w, out = self.w, {}
+    def _weight_views(self, store: bool = False) -> dict:
+        (w, blocks), out = self._view_source(store), {}
         out["img_in.weight"], out["img_in.bias"] = w["img_in_w"], w["img_in_b"]
         out["txt_norm.weight"] = w["txt_norm_w"]
         out["txt_in.weight"], out["txt_in.bias"] = w["txt_in_w"], w["txt_in_b"]
@@ -120,7 +123,7 @@ class QwenImageB200(FusedMMDiTBase):
         out[p + "linear_2.weight"], out[p + "linear_2.bias"] = w["t2_w"], w["t2_b"]
         out["norm_out.linear.weight"], out["norm_out.linear.bias"] = w["norm_out_w"], w["norm_out_b"]
         out["proj_out.weight"], out["proj_out.bias"] = w["proj_out_w"], w["proj_out_b"]
-        return self._double_weight_views(out)
+        return self._double_weight_views(out, w, blocks)
 
     def _embed_table(self) -> dict:
         return {"img_in": ("img_in", 0, self.C_in), "txt_in": ("txt_in", 1, self.J)}
@@ -190,7 +193,7 @@ class QwenImageB200(FusedMMDiTBase):
         lib.timestep_sinusoid(t32, 1000.0, ws["sin"])
         lib.gemv_act(ws["sin"], w["t1_w"], w["t1_b"], ws["t1"], act=0)
         lib.gemv_act(ws["t1"], w["t2_w"], w["t2_b"], ws["temb"], act=1)
-        if self._sharded is None:  # all 2L modulation linears in one launch; sharded weights produce them block by block
+        if self._blk_rings is None:  # all 2L modulation linears in one launch; ringed weights produce them block by block
             lib.gemv_act(ws["temb"], w["mod_w"].view(L * 2 * 6 * D, D), w["mod_b"].view(-1), ws["mods"], act=1)
             self._mod_lora_fwd(ws, ws["temb"])
         lib.gemv_act(ws["temb"], w["norm_out_w"], w["norm_out_b"], ws["fmod"], act=1)

@@ -16,6 +16,9 @@ parallel mode.  B200-first layout instead of FSDP's per-module flat parameters:
     all-gather runs kernels that would) and no rank waits
     for another.  `gather="nccl"` (or QFX_SHARD_GATHER=nccl, or ranks on different hosts) keeps the all_gather_into_tensor path;
   * kernels keep reading plain row-major [out, in] views — the views now point into the gather buffer of the block's slot.
+
+The same two-slot ring (`BlockRing`) has a second fill source: `Nf4Blocks` dequantizes a block's NF4-resident matrices
+(4-bit base checkpoints, nf4.py) into its slot with one kernel launch.
 """
 from __future__ import annotations
 
@@ -28,10 +31,10 @@ ALIGN = 128  # elements (256 B): every packed tensor starts on a TMA-friendly bo
 
 
 class LayerRing:
-    """Stands in for a layer-stacked weight tensor `[L, ...]`: indexing with a layer number returns the view inside the gather
-    buffer that currently holds that layer (and fails loudly if it does not)."""
+    """Stands in for a layer-stacked weight tensor `[L, ...]`: indexing with a layer number returns the view inside the ring
+    buffer slot that currently holds that layer (and fails loudly if it does not)."""
 
-    def __init__(self, owner: "ShardedBlocks", offset: int, shape: tuple):
+    def __init__(self, owner: "BlockRing", offset: int, shape: tuple):
         self.owner, self.offset, self.shape = owner, offset, tuple(shape)
         self.numel = 1
         for d in shape:
@@ -46,25 +49,100 @@ class LayerRing:
         return v[rest] if rest else v
 
 
-class ShardedBlocks:
+class BlockRing:
+    """Two-slot ring of one block kind's weights: block l is filled into slot l & 1 on a side stream (`prefetch`), kernels on
+    the compute stream wait for it (`acquire`), and the slot is refilled only after its last reader has finished (`release`).
+    Subclasses provide the fill source (`_fill(slot, l)`): an all-gather of the ranks' shards, or the NF4 dequantization."""
+
+    def _layout(self, shapes: dict, n_layers: int, dev, dtype) -> int:
+        """One LayerRing view per tensor, each starting on an ALIGN boundary of the slot.  Returns the elements a slot needs."""
+        self.L, self.dev, self.dtype, self.cuda = n_layers, dev, dtype, dev.type == "cuda"
+        off, self.rings = 0, {}
+        for name, shape in shapes.items():
+            self.rings[name] = LayerRing(self, off, shape)
+            off += -(-self.rings[name].numel // ALIGN) * ALIGN
+        return off
+
+    def _alloc_slots(self, n_blk: int):
+        self.gbuf = torch.zeros(2, n_blk, device=self.dev, dtype=self.dtype)
+        self.in_slot = [None, None]
+        if self.cuda:
+            self.comm = torch.cuda.Stream(device=self.dev)
+            self.ready = [torch.cuda.Event(), torch.cuda.Event()]     # fill of the slot finished (comm stream)
+            self.released = [torch.cuda.Event(), torch.cuda.Event()]  # last reader of the slot finished (compute stream)
+            for e in self.released:
+                e.record()
+        self.pending = [False, False]
+
+    def _fill(self, s: int, l: int):
+        raise NotImplementedError
+
+    # ------------------------------------------------------------------------------------------------------------
+    def slot_of(self, l: int) -> int:
+        s = l & 1
+        if self.in_slot[s] != l:
+            raise RuntimeError(f"block {l} is not resident (slot {s} holds {self.in_slot[s]}): call acquire({l}) first")
+        return s
+
+    def prefetch(self, l: int):
+        """Start filling block l into its slot (no-op if it is there already or l is out of range)."""
+        if l < 0 or l >= self.L or self.in_slot[l & 1] == l:
+            return
+        s = l & 1
+        if self.cuda:
+            self.comm.wait_event(self.released[s])  # the previous occupant's kernels have finished reading
+            with torch.cuda.stream(self.comm):
+                self._fill(s, l)
+                self.ready[s].record(self.comm)
+            self.pending[s] = True
+        else:
+            self._fill(s, l)
+        self.in_slot[s] = l
+
+    def acquire(self, l: int):
+        """Make block l's weights valid for kernels on the current stream."""
+        self.prefetch(l)
+        s = l & 1
+        if self.cuda and self.pending[s]:
+            torch.cuda.current_stream().wait_event(self.ready[s])
+            self.pending[s] = False
+
+    def release(self, l: int):
+        """The kernels of block l have been enqueued on the current stream; its slot may be refilled once they finish."""
+        if self.cuda:
+            self.released[l & 1].record(torch.cuda.current_stream())
+
+    def join(self):
+        """The current stream waits for everything issued on the side stream (the end of a captured region must join every stream
+        that forked from it)."""
+        if self.cuda:
+            torch.cuda.current_stream().wait_stream(self.comm)
+
+    def reset(self):
+        """Forget what the slots hold; the next fills wait for everything enqueued so far on the current stream.  A forward that
+        starts here fills the same blocks whether it runs eagerly or is captured into a CUDA graph and replayed, and under capture
+        the side stream forks from the capturing stream through events recorded inside the capture (and joins it again in
+        `acquire`)."""
+        self.in_slot, self.pending = [None, None], [False, False]
+        if self.cuda:
+            for e in self.released:
+                e.record(torch.cuda.current_stream())
+
+
+class ShardedBlocks(BlockRing):
     def __init__(self, stacked: dict, n_layers: int, group=None, gather: str = "auto"):
         """stacked: {name: tensor [L, ...]} (full copies; released by the caller afterwards).
         gather: "auto" (peer copies when every rank is a CUDA device of this host, else NCCL), "peer", or "nccl"."""
         self.group = group
         self.world = dist.get_world_size(group) if dist.is_initialized() else 1
         self.rank = dist.get_rank(group) if dist.is_initialized() else 0
-        self.L = n_layers
         any_t = next(iter(stacked.values()))
-        self.dev, self.dtype = any_t.device, any_t.dtype
-        off, self.rings = 0, {}
-        for name, t in stacked.items():
+        for t in stacked.values():
             assert t.shape[0] == n_layers
-            self.rings[name] = LayerRing(self, off, t.shape[1:])
-            off += -(-self.rings[name].numel // ALIGN) * ALIGN
+        off = self._layout({name: t.shape[1:] for name, t in stacked.items()}, n_layers, any_t.device, any_t.dtype)
         q = self.world * ALIGN
         self.n_blk = -(-off // q) * q
         self.n_shard = self.n_blk // self.world
-        self.cuda = self.dev.type == "cuda"
         self.gather = self._pick_gather(os.environ.get("QFX_SHARD_GATHER", gather))
         self._peer_buf, self._peer_ptrs = None, None
         if self.gather == "peer":
@@ -80,41 +158,11 @@ class ShardedBlocks:
             a, b = max(lo, r.offset), min(hi, r.offset + r.numel)
             if a < b:
                 self.shard[:, a - lo: b - lo] = t.reshape(n_layers, -1)[:, a - r.offset: b - r.offset]
-        self.gbuf = torch.zeros(2, self.n_blk, device=self.dev, dtype=self.dtype)
-        self.in_slot = [None, None]
+        self._alloc_slots(self.n_blk)
         if self.gather == "peer":
             self._open_peers()
-        if self.cuda:
-            self.comm = torch.cuda.Stream(device=self.dev)
-            self.ready = [torch.cuda.Event(), torch.cuda.Event()]     # gather into slot finished (comm stream)
-            self.released = [torch.cuda.Event(), torch.cuda.Event()]  # last reader of the slot finished (compute stream)
-            for e in self.released:
-                e.record()
-        self.pending = [False, False]
 
-    # ------------------------------------------------------------------------------------------------------------
-    def slot_of(self, l: int) -> int:
-        s = l & 1
-        if self.in_slot[s] != l:
-            raise RuntimeError(f"block {l} is not resident (slot {s} holds {self.in_slot[s]}): call acquire({l}) first")
-        return s
-
-    def prefetch(self, l: int):
-        """Start gathering block l into its slot (no-op if it is there already or l is out of range)."""
-        if l < 0 or l >= self.L or self.in_slot[l & 1] == l:
-            return
-        s = l & 1
-        if self.cuda:
-            self.comm.wait_event(self.released[s])  # the previous occupant's kernels have finished reading
-            with torch.cuda.stream(self.comm):
-                self._gather(s, l)
-                self.ready[s].record(self.comm)
-            self.pending[s] = True
-        else:
-            self._gather(s, l)
-        self.in_slot[s] = l
-
-    def _gather(self, s: int, l: int):
+    def _fill(self, s: int, l: int):
         if self.world == 1:
             self.gbuf[s].copy_(self.shard[l])
         elif self.gather == "peer":
@@ -168,15 +216,20 @@ class ShardedBlocks:
             self.shard = None
             self._peer_buf.free()
 
-    def acquire(self, l: int):
-        """Make block l's weights valid for kernels on the current stream."""
-        self.prefetch(l)
-        s = l & 1
-        if self.cuda and self.pending[s]:
-            torch.cuda.current_stream().wait_event(self.ready[s])
-            self.pending[s] = False
 
-    def release(self, l: int):
-        """The kernels of block l have been enqueued on the current stream; its slot may be refilled once they finish."""
-        if self.cuda:
-            self.released[l & 1].record(torch.cuda.current_stream())
+class Nf4Blocks(BlockRing):
+    """NF4-resident frozen weights: every NF4 matrix of a block kind lives as layer-stacked codes + fp32 absmax (nf4.py); a block's
+    bf16 matrices are produced in its ring slot by ONE qfx_nf4_dequant launch right before it runs.  Kernels read the same
+    row-major [out, in] bf16 views as for resident or sharded weights."""
+
+    def __init__(self, stacks: dict, n_layers: int, blocksize: int):
+        """stacks: {name: (codes uint8 [L, ..., in/2], absmax fp32 [L, n/blocksize], bf16 shape of one layer)}."""
+        codes0 = next(iter(stacks.values()))[0]
+        off = self._layout({k: shape for k, (_, _, shape) in stacks.items()}, n_layers, codes0.device, torch.bfloat16)
+        self.stacks, self.blocksize = stacks, blocksize
+        self._alloc_slots(off)
+
+    def _fill(self, s: int, l: int):
+        from . import lib
+        lib.nf4_dequant([(c[l].reshape(-1), a[l].reshape(-1), self.gbuf[s, self.rings[k].offset: self.rings[k].offset + self.rings[k].numel],
+                          self.blocksize) for k, (c, a, _) in self.stacks.items()])
