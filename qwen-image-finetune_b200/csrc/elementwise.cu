@@ -707,6 +707,8 @@ static int dispatch_nv(int D, F&& f) {
   return -1;
 }
 
+static bool aligned(const void* p, uintptr_t bytes) { return (uintptr_t)p % bytes == 0; }  // a null (unused) operand passes
+
 extern "C" int qfx_ln_modulate_fwd_pair(const void* x, int64_t ldx, void* y, int64_t ldy, const void* shift, const void* scale,
                                         int64_t ldmod, int rows_per_batch, float* mean, float* rstd, int M, int D, float eps,
                                         int split, const void* shift1, const void* scale1, int rows_per_batch1, void* stream) {
@@ -736,6 +738,13 @@ extern "C" int qfx_ln_modulate_bwd_pair(const void* dy, int64_t lddy, const void
   QFX_CHECK_ARG(D % 256 == 0, "qfx_ln_modulate_bwd: bad dims");
   QFX_CHECK_ARG(split >= M || (scale1 && rows_per_batch1 > 0 && ((gate1 != nullptr) == (gate != nullptr))),
                 "qfx_ln_modulate_bwd_pair: second group needs scale (and a gate iff the first group has one)");
+  // every operand is accessed in 16-byte vectors: 8-element leading dimensions and 16-byte aligned bases
+  QFX_CHECK_ARG(lddy % 8 == 0 && ldx % 8 == 0 && ldmod % 8 == 0 && lddx % 8 == 0 && (!dres || lddres % 8 == 0) &&
+                    (!dx_gated || (ldgate % 8 == 0 && lddxg % 8 == 0)),
+                "qfx_ln_modulate_bwd_pair: leading dimensions must be multiples of 8 elements");
+  QFX_CHECK_ARG(aligned(dy, 16) && aligned(x, 16) && aligned(scale, 16) && aligned(scale1, 16) && aligned(dres, 16) &&
+                    aligned(dx, 16) && (!dx_gated || (aligned(gate, 16) && aligned(gate1, 16) && aligned(dx_gated, 16))),
+                "qfx_ln_modulate_bwd_pair: operands must be 16-byte aligned");
   return dispatch_nv(D, [&](auto w, auto vpt) {
     constexpr int W = decltype(w)::value, RPC = 8 / W;
     ln_modulate_bwd_kernel<W, decltype(vpt)::value><<<(M + RPC - 1) / RPC, 256, 0, (cudaStream_t)stream>>>(
@@ -792,6 +801,7 @@ extern "C" int qfx_qk_norm_rope_fwd_pair(const void* qkv, int64_t ldqkv, const v
                                          int s_offset, int S, int H, float eps, int round_mid, int split, const void* wq1,
                                          const void* wk1, int tokens_per_sample1, int s_offset1, void* stream) {
   QFX_CHECK_ARG(split >= tokens || (wq1 && wk1 && tokens_per_sample1 > 0), "qfx_qk_norm_rope_fwd_pair: second group incomplete");
+  QFX_CHECK_ARG(ldqkv % 4 == 0 && aligned(qkv, 8), "qfx_qk_norm_rope_fwd_pair: qkv needs an 8-byte aligned base and ldqkv %% 4 == 0");
   const int blocks = (tokens * H + 7) / 8;
   if (round_mid)
     qk_norm_rope_fwd_kernel<true><<<blocks, 256, 0, (cudaStream_t)stream>>>(
@@ -817,6 +827,8 @@ extern "C" int qfx_qk_norm_rope_bwd_pair(void* dQ, const void* dK, const void* d
                                          int round_mid, int split, const void* wq1, const void* wk1, int tokens_per_sample1,
                                          int s_offset1, int clear_dq, void* stream) {
   QFX_CHECK_ARG(split >= tokens || (wq1 && wk1 && tokens_per_sample1 > 0), "qfx_qk_norm_rope_bwd_pair: second group incomplete");
+  QFX_CHECK_ARG(ldqkv % 4 == 0 && lddqkv % 4 == 0 && aligned(qkv, 8) && aligned(dqkv, 8) && aligned(dQ, 16),
+                "qfx_qk_norm_rope_bwd_pair: qkv / dqkv need 8-byte aligned bases and leading dimensions %% 4 == 0");
   const int blocks = (tokens * H + 7) / 8;
   if (round_mid)
     qk_norm_rope_bwd_kernel<true><<<blocks, 256, 0, (cudaStream_t)stream>>>(
@@ -915,6 +927,8 @@ extern "C" int qfx_attn_delta_pair(const void* O, int64_t ldo, const void* dO, i
                                    int tokens, int tokens_per_sample, int s_offset, int S, int H, int split, int tokens_per_sample1,
                                    int s_offset1, void* stream) {
   QFX_CHECK_ARG(split >= tokens || tokens_per_sample1 > 0, "qfx_attn_delta_pair: second group incomplete");
+  QFX_CHECK_ARG(ldo % 4 == 0 && lddo % 4 == 0 && aligned(O, 8) && aligned(dO, 8),
+                "qfx_attn_delta_pair: O / dO need 8-byte aligned bases and leading dimensions %% 4 == 0");
   attn_delta_kernel<<<(tokens * H + 7) / 8, 256, 0, (cudaStream_t)stream>>>((const bf16*)O, ldo, (const bf16*)dO, lddo, delta,
                                                                             (bf16*)dO_joint, tokens, tokens_per_sample, s_offset,
                                                                             S, H, split, tokens_per_sample1, s_offset1);

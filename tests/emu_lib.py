@@ -1,10 +1,10 @@
 """TEST INFRASTRUCTURE ONLY — plain-PyTorch (fp32 math, bf16 storage) emulation of every `qflux_b200.lib` entry point.
 
-Two uses:
-  * `-m "not gpu"` tests monkey-patch it over `qflux_b200.lib` to exercise the host-side orchestration (launch order,
-    operand wiring, LoRA registry, gradient offsets) of the fused model on CPU against the oracle;
-  * `-m gpu` tests use the same functions as the "plain PyTorch fp32 reference of the same op" for each CUDA kernel.
-It is never imported by the product package.
+`-m "not gpu"` tests monkey-patch it over `qflux_b200.lib` to exercise the host-side orchestration (launch order, operand wiring,
+LoRA registry, gradient offsets) of the fused model on CPU against the oracle.  The emulation is held to the kernels it stands in
+for by tests/test_glue_kernels.py (tools/glue_check.py, `-m gpu`): element by element on the same inputs, bit-identical for data
+movement and within a stated rounding-flip bound elsewhere.  The `-m gpu` kernel cases themselves compare against independent
+fp64 references, not against this file.  It is never imported by the product package.
 """
 from __future__ import annotations
 
@@ -336,8 +336,10 @@ def qk_norm_rope_fwd_pair(qkv, g0, g1, split, rope, Q, K, V, eps=1e-6, round_mid
 def qk_norm_rope_bwd_pair(dQ, dK, dV, qkv, g0, g1, split, rope, dqkv, eps=1e-6, round_mid=True, clear_dq=False):
     for (wq, wk, tps, so), sl in ((g0, slice(0, split)), (g1, slice(split, None))):
         qk_norm_rope_bwd(dQ, dK, dV, qkv[sl], wq, wk, rope, dqkv[sl], tps, so, eps=eps, round_mid=round_mid)
-    if clear_dq:
-        dQ.zero_()
+    if clear_dq:  # like the kernel: only the positions the two groups read are zeroed (qfx.h asks the groups to cover all of S)
+        for (_, _, tps, so), sl in ((g0, slice(0, split)), (g1, slice(split, None))):
+            if qkv[sl].shape[0]:
+                dQ[:qkv[sl].shape[0] // tps, :, so:so + tps] = 0
 
 
 def attn_delta_pair(O, dO, delta, g0, g1, split, dO_joint=None):
