@@ -34,6 +34,9 @@ int qfx_version(void);
  *
  * The LoRA factor pair (A2,B2) is appended to the K loop of the SAME tensor-core contraction (rank padded to a
  * multiple of 64 with zeros by the caller), so one register accumulator receives base + low-rank update.
+ * alpha scales the accumulator for the BIAS, ADD, DGELU and ATTN_DO epilogues only; GELU and RESID_GATE refuse alpha != 1.
+ * out, out2, bias, resid, gate and aux are accessed as 16-byte vectors: their bases must be 16-byte aligned and their leading
+ * dimensions multiples of 8 elements.
  */
 #define QFX_MAX_PROBLEMS 6
 
@@ -91,7 +94,9 @@ int qfx_zero_rows(void* out, int64_t ld, int ncols, const int* ranges, int n_ran
  * Forward writes O token-major into two row groups: rows with joint position s < split of sample b go to
  * out0[(b*rows0 + s)*ld0 + h*128 ..], the others to out1[(b*rows1 + s - split)*ld1 + h*128 ..]; lse is the log2-domain
  * log-sum-exp [B,H,S].  Backward: dQ_accum is fp32 [B,H,S,128], zeroed by the caller (every key tile adds into it);
- * delta = rowsum(dO * O) [B,H,S]. */
+ * delta = rowsum(dO * O) [B,H,S].  txt_len needs 0 < split <= S.  Forward: rows0 >= split, rows1 >= S - split, out0 / out1
+ * 16-byte aligned with ld0 / ld1 >= H*128 and multiples of 8.  A query tile of only padding rows (every position >= kv_len[b]
+ * and >= split) gets O = 0 and lse = 0. */
 int qfx_attn_fwd(const void* Q, const void* K, const void* V, void* out0, int64_t ld0, int rows0, void* out1, int64_t ld1,
                  int rows1, int split, float* lse, const int* kv_len, const int* txt_len, int B, int H, int S,
                  float softmax_scale, void* stream);

@@ -233,6 +233,10 @@ extern "C" int qfx_attn_bwd(const void* Q, const void* K, const void* V, const v
                             float* dQ_accum, void* dK, void* dV, const int* kv_len, const int* txt_len, int split, int B, int H,
                             int S, float softmax_scale, void* stream) {
   QFX_CHECK_ARG(B > 0 && H > 0 && S > 0 && dQ_accum && dK && dV && lse && delta, "qfx_attn_bwd: bad arguments");
+  QFX_CHECK_ARG(!txt_len || (split > 0 && split <= S), "qfx_attn_bwd: txt_len needs 0 < split <= S (split=%d S=%d)", split, S);
+  // dQ is reduced into as 8-byte pairs, dK / dV are stored as 4-byte pairs
+  QFX_CHECK_ARG(((uintptr_t)dQ_accum & 7) == 0 && ((uintptr_t)dK & 3) == 0 && ((uintptr_t)dV & 3) == 0,
+                "qfx_attn_bwd: dQ_accum must be 8-byte aligned, dK / dV 4-byte aligned");
   AttnBwdParams P;
   memset(&P, 0, sizeof(P));
   int rc;

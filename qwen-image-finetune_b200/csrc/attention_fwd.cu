@@ -200,6 +200,14 @@ extern "C" int qfx_attn_fwd(const void* Q, const void* K, const void* V, void* o
                             int64_t ld1, int rows1, int split, float* lse, const int* kv_len, const int* txt_len, int B, int H,
                             int S, float softmax_scale, void* stream) {
   QFX_CHECK_ARG(B > 0 && H > 0 && S > 0 && out0 && (split >= S || out1), "qfx_attn_fwd: bad arguments");
+  QFX_CHECK_ARG(split >= 0 && rows0 >= (split < S ? split : S) && (split >= S || rows1 >= S - split),
+                "qfx_attn_fwd: row groups too short (split=%d S=%d rows0=%d rows1=%d)", split, S, rows0, rows1);
+  QFX_CHECK_ARG(!txt_len || (split > 0 && split <= S), "qfx_attn_fwd: txt_len needs 0 < split <= S (split=%d S=%d)", split, S);
+  // rows are stored as 4-byte pairs and, in padding query tiles, as 16-byte vectors
+  QFX_CHECK_ARG(ld0 % 8 == 0 && ld0 >= (int64_t)H * ATT_D && ((uintptr_t)out0 & 15) == 0 &&
+                    (split >= S || (ld1 % 8 == 0 && ld1 >= (int64_t)H * ATT_D && ((uintptr_t)out1 & 15) == 0)),
+                "qfx_attn_fwd: out0 / out1 must be 16-byte aligned with leading dimensions >= H*128 and multiples of 8 (ld0=%lld ld1=%lld)",
+                (long long)ld0, (long long)ld1);
   AttnFwdParams P;
   memset(&P, 0, sizeof(P));
   int rc;

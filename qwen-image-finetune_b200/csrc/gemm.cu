@@ -428,6 +428,40 @@ extern "C" int qfx_gemm_bf16(const qfx_gemm_problem* probs, int nprob, int N, in
   QFX_CHECK_ARG((bn == 64 || bn == 128 || bn == 192 || bn == 256) && N % bn == 0, "qfx_gemm_bf16: N=%d block_n=%d", N, bn);
   QFX_CHECK_ARG(!(trans_b && lora_group_n), "qfx_gemm_bf16: lora_group_n only with trans_b=0");
   QFX_CHECK_ARG(lora_group_n == 0 || lora_group_n % bn == 0, "qfx_gemm_bf16: lora_group_n %% block_n != 0");
+  QFX_CHECK_ARG(alpha == 1.f || (epilogue != QFX_EPI_GELU && epilogue != QFX_EPI_RESID_GATE),
+                "qfx_gemm_bf16: the GELU and RESID_GATE epilogues take alpha = 1 only (alpha=%g)", alpha);
+
+  // Every problem is validated before any tensor map is encoded: a refusal never depends on the driver.  The epilogue operands are
+  // read and written as 16-byte vectors, so their bases and leading dimensions must allow that.
+  auto al16 = [](const void* p) { return ((uintptr_t)p & 15) == 0; };
+  for (int i = 0; i < nprob; ++i) {
+    const qfx_gemm_problem& s = probs[i];
+    QFX_CHECK_ARG(s.M > 0 && s.A && s.B && s.out, "qfx_gemm_bf16: problem %d has null/empty operands", i);
+    QFX_CHECK_ARG(s.lda % 8 == 0 && s.ldb % 8 == 0 && s.ldo % 8 == 0, "qfx_gemm_bf16: leading dims must be multiples of 8");
+    QFX_CHECK_ARG(s.kb2 >= 0 && s.a2_col0 >= 0, "qfx_gemm_bf16: problem %d: kb2=%d a2_col0=%d", i, s.kb2, s.a2_col0);
+    if (s.kb2 > 0) QFX_CHECK_ARG(s.A2 && s.B2 && s.lda2 % 8 == 0 && s.ldb2 % 8 == 0, "qfx_gemm_bf16: bad LoRA operands");
+    QFX_CHECK_ARG(!s.row_tiles || s.n_row_tiles > 0, "qfx_gemm_bf16: row_tiles without n_row_tiles");
+    if (epilogue == QFX_EPI_GELU) QFX_CHECK_ARG(s.out2 && s.ldo2 % 8 == 0, "qfx_gemm_bf16: GELU epilogue needs out2");
+    if (epilogue == QFX_EPI_RESID_GATE) QFX_CHECK_ARG(s.resid && s.gate && s.ldr % 8 == 0 && s.ldg % 8 == 0, "qfx_gemm_bf16: RESID_GATE epilogue needs resid+gate");
+    if (epilogue == QFX_EPI_ADD) QFX_CHECK_ARG(s.resid && s.ldr % 8 == 0, "qfx_gemm_bf16: ADD epilogue needs resid");
+    if (epilogue == QFX_EPI_DGELU) QFX_CHECK_ARG(s.aux && s.ldaux % 8 == 0, "qfx_gemm_bf16: DGELU epilogue needs aux");
+    if (epilogue == QFX_EPI_ATTN_DO) {
+      QFX_CHECK_ARG(s.aux && s.ldaux % 8 == 0 && s.delta && s.attn_H * 128 == N && s.attn_S > 0 && s.rows_per_batch > 0 && !s.row_tiles,
+                    "qfx_gemm_bf16: ATTN_DO epilogue needs aux (O), delta, attn_H*128 == N, attn_S, rows_per_batch (dense rows only)");
+      QFX_CHECK_ARG(s.s_offset >= 0 && s.s_offset + s.rows_per_batch <= s.attn_S,
+                    "qfx_gemm_bf16: ATTN_DO problem %d: joint positions [%d, %d) outside attn_S=%d", i, s.s_offset,
+                    s.s_offset + s.rows_per_batch, s.attn_S);
+      QFX_CHECK_ARG(i == 0 || (s.delta == probs[0].delta && s.attn_S == probs[0].attn_S && s.attn_H == probs[0].attn_H),
+                    "qfx_gemm_bf16: ATTN_DO row groups must share delta / attn_S / attn_H");
+    }
+    const bool has_out2 = s.out2 && (epilogue == QFX_EPI_GELU || epilogue == QFX_EPI_RESID_GATE || epilogue == QFX_EPI_ATTN_DO);
+    if (has_out2) QFX_CHECK_ARG(s.ldo2 % 8 == 0, "qfx_gemm_bf16: problem %d: ldo2=%lld must be a multiple of 8", i, (long long)s.ldo2);
+    QFX_CHECK_ARG(al16(s.out) && al16(s.bias) && (!has_out2 || al16(s.out2)) &&
+                      (!(epilogue == QFX_EPI_RESID_GATE || epilogue == QFX_EPI_ADD) || al16(s.resid)) &&
+                      (epilogue != QFX_EPI_RESID_GATE || al16(s.gate)) &&
+                      (!(epilogue == QFX_EPI_DGELU || epilogue == QFX_EPI_ATTN_DO) || al16(s.aux)),
+                  "qfx_gemm_bf16: problem %d: out / out2 / bias / resid / gate / aux must be 16-byte aligned", i);
+  }
 
   GemmParams P;
   memset(&P, 0, sizeof(P));
@@ -448,8 +482,6 @@ extern "C" int qfx_gemm_bf16(const qfx_gemm_problem* probs, int nprob, int N, in
   for (int i = 0; i < nprob; ++i) {
     const qfx_gemm_problem& s = probs[i];
     GemmProb& d = P.p[i];
-    QFX_CHECK_ARG(s.M > 0 && s.A && s.B && s.out, "qfx_gemm_bf16: problem %d has null/empty operands", i);
-    QFX_CHECK_ARG(s.lda % 8 == 0 && s.ldb % 8 == 0 && s.ldo % 8 == 0, "qfx_gemm_bf16: leading dims must be multiples of 8");
     int rc = make_2d(&d.tmA, s.A, (uint64_t)K, (uint64_t)s.M, s.lda, BK, BM);
     if (rc) return rc;
     if (!trans_b)
@@ -460,7 +492,6 @@ extern "C" int qfx_gemm_bf16(const qfx_gemm_problem* probs, int nprob, int N, in
     d.kb2 = s.kb2;
     d.a2_col0 = s.a2_col0;
     if (s.kb2 > 0) {
-      QFX_CHECK_ARG(s.A2 && s.B2 && s.lda2 % 8 == 0 && s.ldb2 % 8 == 0, "qfx_gemm_bf16: bad LoRA operands");
       const int groups = lora_group_n ? N / lora_group_n : 1;
       rc = make_2d(&d.tmA2, s.A2, (uint64_t)(s.a2_col0 + 64 * s.kb2 * groups), (uint64_t)s.M, s.lda2, BK, BM);
       if (rc) return rc;
@@ -480,18 +511,8 @@ extern "C" int qfx_gemm_bf16(const qfx_gemm_problem* probs, int nprob, int N, in
     d.aux = (const bf16*)s.aux;
     d.ldo = s.ldo; d.ldo2 = s.ldo2; d.ldr = s.ldr; d.ldg = s.ldg; d.ldaux = s.ldaux;
     d.row_tiles = s.row_tiles;
-    QFX_CHECK_ARG(!s.row_tiles || s.n_row_tiles > 0, "qfx_gemm_bf16: row_tiles without n_row_tiles");
-    if (epilogue == QFX_EPI_GELU) QFX_CHECK_ARG(s.out2 && s.ldo2 % 8 == 0, "qfx_gemm_bf16: GELU epilogue needs out2");
-    if (epilogue == QFX_EPI_RESID_GATE) QFX_CHECK_ARG(s.resid && s.gate && s.ldr % 8 == 0 && s.ldg % 8 == 0, "qfx_gemm_bf16: RESID_GATE epilogue needs resid+gate");
-    if (epilogue == QFX_EPI_ADD) QFX_CHECK_ARG(s.resid && s.ldr % 8 == 0, "qfx_gemm_bf16: ADD epilogue needs resid");
-    if (epilogue == QFX_EPI_DGELU) QFX_CHECK_ARG(s.aux && s.ldaux % 8 == 0, "qfx_gemm_bf16: DGELU epilogue needs aux");
-    if (epilogue == QFX_EPI_ATTN_DO)
-      QFX_CHECK_ARG(s.aux && s.ldaux % 8 == 0 && s.delta && s.attn_H * 128 == N && s.attn_S > 0 && s.rows_per_batch > 0 && !s.row_tiles,
-                    "qfx_gemm_bf16: ATTN_DO epilogue needs aux (O), delta, attn_H*128 == N, attn_S, rows_per_batch (dense rows only)");
     d.s_offset = s.s_offset;
     if (epilogue == QFX_EPI_ATTN_DO) {
-      QFX_CHECK_ARG(i == 0 || (s.delta == P.delta && s.attn_S == P.attn_S && s.attn_H == P.attn_H),
-                    "qfx_gemm_bf16: ATTN_DO row groups must share delta / attn_S / attn_H");
       P.delta = s.delta; P.attn_S = s.attn_S; P.attn_H = s.attn_H;
     }
     int tm = (s.M + BM - 1) / BM;

@@ -35,6 +35,8 @@ def _gelu_grad(u):
 
 
 def gemm(problems, N, K, *, trans_b=False, epilogue=EPI_BIAS, alpha=1.0, lora_group_n=0, block_n=0):
+    # like qfx_gemm_bf16: alpha scales the accumulator of BIAS / ADD / DGELU / ATTN_DO only
+    assert alpha == 1.0 or epilogue not in (EPI_GELU, EPI_RESID_GATE), "the GELU and RESID_GATE epilogues take alpha = 1 only"
     for p in problems:
         A, W = p.A.float(), p.B.float()
         acc = A @ (W if trans_b else W.t())
@@ -58,7 +60,7 @@ def gemm(problems, N, K, *, trans_b=False, epilogue=EPI_BIAS, alpha=1.0, lora_gr
         elif epilogue == EPI_RESID_GATE:
             y = (acc + b).to(BF).float()
             rpb = p.rows_per_batch or A.shape[0]
-            g = p.gate.float().repeat_interleave(rpb, 0)
+            g = p.gate.float().repeat_interleave(rpb, 0)[:A.shape[0]]  # row -> gate row // rows_per_batch, as the kernel
             p.out.copy_((p.resid.float() + (g * y).to(BF).float()).to(BF))
             if p.out2 is not None:
                 p.out2.copy_(y.to(BF))
