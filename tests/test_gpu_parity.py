@@ -4,7 +4,8 @@ cases can also be run stand-alone (one subprocess per case) when debugging on a 
 
 Tolerances (relative L2, the reference's own convention tests/src/models/test_qwen_custom.py:550):
   single kernels: 5e-3 (bf16 output rounding is 1.7e-3 RMS);   fused step vs fp32 oracle: pred 2e-2 and not worse than
-  1.25x the bf16 eager oracle's own error, LoRA grads 3e-2, |loss diff| <= 1e-2 relative to max(1, loss).
+  1.25x the bf16 eager oracle's own error, LoRA grads 3e-2 pooled and, per tensor, 1.5x the bf16 eager oracle's error for that
+  tensor + 2e-3 (at most 3e-2), |loss diff| <= 1e-2 relative to max(1, loss).
 """
 import os
 import sys
@@ -74,6 +75,8 @@ def test_fused_step_vs_oracle(name):
         return
     assert r["pred_vs_fp32"] < 2e-2 and r["pred_vs_fp32"] < 1.25 * r["bf16oracle_pred_vs_fp32"] + 1e-3
     assert r["grad_vs_fp32"] < 3e-2
+    # and every LoRA tensor on its own: within 1.5x the bf16 oracle's error for that tensor + 2e-3, and under 3e-2
+    assert not r["grad_tensor_fail"], r["grad_tensor_fail"]
     assert r["loss_rel"] < 1e-2
     assert r["fast_vs_autograd"] < 5e-3
 

@@ -9,6 +9,7 @@ import time
 
 sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
 from harness import main, rel_l2  # noqa: E402
+from lora_grad_check import eager_sdpa, per_tensor  # noqa: E402
 
 import torch  # noqa: E402
 
@@ -51,6 +52,13 @@ def inputs(B, hw, T, J, seed=0):
                 u=torch.tensor([0.5, 0.25, 0.125, 0.75][:B]))  # sigma .5/.75/.875/.25: exact in bf16
 
 
+def _grad_per_tensor(res, gb, g_o, g_h):
+    """Each LoRA gradient tensor of the fused step against the fp32 oracle, scaled by the bf16 oracle's own error for that tensor
+    (lora_grad_check.per_tensor): a pooled norm over all tensors would hide a wrong small one."""
+    pt = per_tensor(gb, g_o, g_h)
+    res["grad_tensor_fail"], res["grad_worst_ratio"] = pt["fail"], pt["worst_ratio"]
+
+
 def step_parity(H=2, L=2, J=128, B=2, hw=4, T=24, r=4, targets=("to_q", "to_k", "to_v", "to_out.0"), bf16_oracle=True):
     from oracle import mmdit_oracle as mo
     from qflux_b200.train_step import QwenImageEditStep
@@ -87,13 +95,15 @@ def step_parity(H=2, L=2, J=128, B=2, hw=4, T=24, r=4, targets=("to_q", "to_k", 
     if bf16_oracle:
         orc.zero_grad()
         orc16 = orc.bfloat16()
-        loss_h, pred_h = mo.qwen_compute_loss(orc16, **x)
-        loss_h.backward()
+        with eager_sdpa():
+            loss_h, pred_h = mo.qwen_compute_loss(orc16, **x)
+            loss_h.backward()
         g_h = {n: (p.grad.float() if p.grad is not None else torch.zeros_like(p).float()) for n, p in orc16.named_parameters() if p.requires_grad}
         res["bf16oracle_pred_vs_fp32"] = rel_l2(pred_h.float(), pred_o)
         res["pred_vs_bf16oracle"] = rel_l2(pred_b, pred_h.float())
         num = sum(((g_h[n] - g_o[n]).double() ** 2).sum() for n in g_o)
         res["bf16oracle_grad_vs_fp32"] = float((num / den).sqrt())
+        _grad_per_tensor(res, gb, g_o, g_h)
     res["err"] = max(res["pred_vs_fp32"], res["grad_vs_fp32"])
     return res
 
@@ -425,10 +435,14 @@ def flux_step_parity(H=2, L=2, Ls=2, J=64, Pp=64, B=2, hw=4, T=8, r=4,
     res["fast_vs_autograd"] = max(rel_l2(gv[n], gb[n]) for n in gb if gb[n].abs().max() > 0)
     orc.zero_grad()
     orc16 = orc.bfloat16()
-    _, pred_h = mo.flux_compute_loss_shared(orc16, emb["image_latents"], emb["control_latents"], emb["pooled_prompt_embeds"],
-                                            emb["prompt_embeds"], emb["text_ids"], emb["image_ids"], emb["control_ids"], noise=noise,
-                                            t=t.bfloat16())
+    with eager_sdpa():  # not cuDNN attention: its backward is wrong for this oracle (lora_grad_check.eager_sdpa)
+        loss_h, pred_h = mo.flux_compute_loss_shared(orc16, emb["image_latents"], emb["control_latents"], emb["pooled_prompt_embeds"],
+                                                     emb["prompt_embeds"], emb["text_ids"], emb["image_ids"], emb["control_ids"],
+                                                     noise=noise, t=t.bfloat16())
+        loss_h.backward()
+    g_h = {n: (p.grad.float() if p.grad is not None else torch.zeros_like(p).float()) for n, p in orc16.named_parameters() if p.requires_grad}
     res["bf16oracle_pred_vs_fp32"] = rel_l2(pred_h.float(), pred_o)
+    _grad_per_tensor(res, gb, g_o, g_h)
     res["err"] = max(res["pred_vs_fp32"], res["grad_vs_fp32"])
     return res
 
