@@ -231,6 +231,19 @@ typedef struct {
 int qfx_nf4_dequant(const qfx_nf4_segment* segs, int nseg, void* stream);
 
 /* ------------------------------------------------------------------------------------------------------------------
+ * FP8 frozen weights (float8-e4m3fn base checkpoints without scales, e.g. `*_fp8_e4m3fn` diffusers exports).  One launch expands
+ * up to QFX_FP8_MAX_SEGMENTS tensors (the FP8 matrices of one block) into bf16:  out[i] = bf16(e4m3fn codes[i]), exact for every
+ * finite code (subnormals down to 2^-9 included; -0 gives 0x8000).  n % 16 == 0; codes and out 16-byte aligned.  The segment
+ * table is read on the host and passed by value: no device table, no host synchronisation. */
+#define QFX_FP8_MAX_SEGMENTS 8
+typedef struct {
+  const void* codes;  /* n bytes, one e4m3fn code per element */
+  void* out;          /* n bf16 */
+  int64_t n;
+} qfx_fp8_segment;
+int qfx_fp8_expand(const qfx_fp8_segment* segs, int nseg, void* stream);
+
+/* ------------------------------------------------------------------------------------------------------------------
  * Peer memory for sharded frozen weights (replaces FSDP's per-module all-gather, base_trainer.py:333-382, for the frozen block
  * weights).  A rank's weight shard lives in an allocation made by qfx_peer_alloc; its 64-byte handle is sent to the other ranks
  * of the node (any host transport), which map it with qfx_peer_open.  qfx_peer_copy_async then pulls bytes from a mapped peer

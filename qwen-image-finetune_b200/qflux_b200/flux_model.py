@@ -69,7 +69,7 @@ class FluxB200(FusedMMDiTBase):
     _SINGLE_MATS = {**{nm: grp + "_w" for nm, (grp, _) in _SINGLE_LINEARS.items()}, "norm.linear": "s_mod_w"}
 
     def __init__(self, cfg: FluxB200Config, device="cuda", _host_only: bool = False, frozen_weights="bf16", nf4_blocksize: int = 64):
-        """frozen_weights / nf4_blocksize: as for QwenImageB200 (4-bit base checkpoints)."""
+        """frozen_weights / nf4_blocksize: as for QwenImageB200 (4-bit and float8-e4m3fn base checkpoints)."""
         super().__init__()
         self._init_common(device, _host_only, frozen_weights, nf4_blocksize)
         assert cfg.attention_head_dim == 128, "the sm_90a attention kernels are specialised for head_dim 128"

@@ -23,11 +23,14 @@ def _cfg_get(cfg, k, default=None):
         return getattr(cfg, k, default)
 
 
-def from_reference(ref_model, device=None, _host_only: bool = False):
+def from_reference(ref_model, device=None, _host_only: bool = False, frozen_weights=None):
     """Build the fused model for a loaded reference / diffusers transformer (`QwenImageTransformer2DModel` or
     `FluxTransformer2DModel`): same config, weights copied through the shared state-dict key names, and — when the module already
     carries a PEFT adapter (`peft_config`) — the same adapter with the same factors.  A 4-bit base model (bitsandbytes `Linear4bit`,
-    NF4) gives a model whose block matrices stay NF4-resident (`frozen_weights`, picked per stacked kind from what the state dict holds)."""
+    NF4) gives a model whose block matrices stay NF4-resident (`frozen_weights`, picked per stacked kind from what the state dict holds).
+    frozen_weights="fp8" keeps the block matrices of a float8-e4m3fn checkpoint FP8-resident; they may arrive as float8_e4m3fn or as
+    the exact bf16 upcast that diffusers' `from_pretrained(torch_dtype=bfloat16)` holds (fp8.py).  Any other value is passed to the
+    constructor as given."""
     from . import nf4
     from .flux_model import FluxB200, FluxB200Config
     from .qwen_model import QwenB200Config, QwenImageB200
@@ -53,12 +56,16 @@ def from_reference(ref_model, device=None, _host_only: bool = False):
             raise nf4.QfxError(f"the NF4 block matrices use blocksizes {sorted(sizes)}; the fused layout takes one per model")
         if kinds:
             nf4_kw = dict(frozen_weights=tuple(kinds), nf4_blocksize=sizes.pop())
+    if frozen_weights is not None:
+        nf4_kw["frozen_weights"] = frozen_weights
     dit = M(C(**kw), device=device, _host_only=_host_only, **nf4_kw)
     peft_cfg = getattr(ref_model, "peft_config", None)
     if peft_cfg:
         (name, pc), = list(peft_cfg.items())
         dit.add_adapter(pc, adapter_name=name)
-    if quant or dit.frozen_weights != "bf16":
+    if dit.frozen_weights == "fp8":
+        dit.load_state_dict(sd, strict=True)
+    elif quant or dit.frozen_weights != "bf16":
         dit._load_nf4(plain, quant, strict=True)
     else:
         dit.load_state_dict(sd, strict=True)
@@ -68,7 +75,9 @@ def from_reference(ref_model, device=None, _host_only: bool = False):
 def patch_trainer(trainer, use_fused_step: bool = True, _host_only: bool = False):
     """Swap the hot path of a constructed reference trainer (QwenImageEdit / QwenImageEditPlus / FluxKontext) in place.
 
-    * `trainer.dit` becomes the fused model (weights and adapter taken over from the loaded reference module);
+    * `trainer.dit` becomes the fused model (weights and adapter taken over from the loaded reference module), with FP8-resident
+      block weights when the trainer's config reports `quantization_type == "pretrain_fp8"` (the reference's marker of an FP8
+      checkpoint, config.py `_compute_quantization_type`);
     * `trainer._compute_loss(embeddings)` becomes `QwenImageEditStep.compute_loss` / `FluxKontextStep.compute_loss` (same contract:
       scalar with autograd history to the LoRA parameters), with the loss kind read off `trainer.criterion`;
     * `trainer.b200_step` exposes the fused step for callers that want the no-autograd fast path (`train_step`).
@@ -79,7 +88,8 @@ def patch_trainer(trainer, use_fused_step: bool = True, _host_only: bool = False
     dit = trainer.dit
     if not isinstance(dit, FusedMMDiTBase):
         acc = getattr(trainer, "accelerator", None)
-        dit = from_reference(dit, getattr(acc, "device", None), _host_only)
+        fw = "fp8" if _cfg_get(getattr(trainer, "config", None), "quantization_type") == "pretrain_fp8" else None
+        dit = from_reference(dit, getattr(acc, "device", None), _host_only, frozen_weights=fw)
         trainer.dit = dit
     crit = getattr(trainer, "criterion", None)
     kind = _LOSS_KIND.get(type(crit).__name__, "mse")

@@ -461,6 +461,27 @@ def nf4_dequant(segments):
     check(_nf4(arr, len(segments), cur_stream()), "qfx_nf4_dequant")
 
 
+# ---------------------------------------------------------------------------------------------------- FP8 frozen weights (fp8.py)
+class Fp8Segment(C.Structure):
+    _fields_ = [("codes", C.c_void_p), ("out", C.c_void_p), ("n", C.c_int64)]
+
+
+FP8_MAX_SEGMENTS = 8
+_fp8 = _sig("qfx_fp8_expand", C.POINTER(Fp8Segment), _i, _vp)
+
+
+def fp8_expand(segments):
+    """segments: [(codes float8_e4m3fn or uint8 [n], out bf16 [n])], contiguous; ONE launch fills every out with bf16(codes),
+    exact for every finite code."""
+    arr = (Fp8Segment * len(segments))()
+    for i, (codes, out) in enumerate(segments):
+        require_cuda(codes, out)
+        assert codes.dtype in (torch.float8_e4m3fn, torch.uint8) and out.dtype == torch.bfloat16
+        assert codes.is_contiguous() and out.is_contiguous() and codes.numel() == out.numel()
+        arr[i] = Fp8Segment(codes.data_ptr(), out.data_ptr(), out.numel())
+    check(_fp8(arr, len(segments), cur_stream()), "qfx_fp8_expand")
+
+
 # ---------------------------------------------------------------------------------------------------- peer memory (sharding.py)
 PEER_HANDLE_BYTES = 64
 for _f in ("qfx_peer_alloc", "qfx_peer_free", "qfx_peer_open", "qfx_peer_close", "qfx_peer_copy_async"):

@@ -165,13 +165,16 @@ class FusedMMDiTBase(nn.Module):
         return self.w[grp + "_w"][l, s], self.w[grp + "_b"][l, s]
 
     def _view_source(self, store: bool):
-        """(weights dict, whether block entries are included) for `_weight_views`.  store=True: every block, with the NF4-resident
-        kinds as meta tensors of their bf16 shape — their views' storage offsets address the codes and absmax (load_state_dict)."""
+        """(weights dict, whether block entries are included) for `_weight_views`.  store=True: every block, with the NF4- or
+        FP8-resident kinds as meta tensors of their bf16 shape — their views' storage offsets address the resident storage
+        (load_state_dict)."""
         if not store:
             return self.w, self._blk_rings is None
         w = dict(self.w)
         for k, (codes, _) in self._nf4_store.items():
             w[k] = torch.empty(*codes.shape[:-1], codes.shape[-1] * 2, device="meta", dtype=BF)
+        for k, codes in self._fp8_store.items():
+            w[k] = torch.empty(*codes.shape, device="meta", dtype=BF)
         return w, True
 
     @classmethod
@@ -190,16 +193,20 @@ class FusedMMDiTBase(nn.Module):
     # -----------------------------------------------------------------------------------------------------------------
     def _init_common(self, device, host_only, frozen_weights="bf16", nf4_blocksize=64):
         """frozen_weights: "bf16" (block weights resident in bf16), "nf4" (every stacked block matrix NF4-resident: a 4-bit base
-        checkpoint) or the set of stacked kinds that are (`from_reference` picks what the checkpoint holds)."""
+        checkpoint) or the set of stacked kinds that are (`from_reference` picks what the checkpoint holds), or "fp8" (every stacked
+        block matrix held as float8-e4m3fn bytes: an FP8 base checkpoint without scales)."""
         if not host_only and not torch.cuda.is_available():
             raise lib.QfxError(f"{type(self).__name__} needs a CUDA device (sm_90a); there is no CPU fallback")
-        kinds = () if frozen_weights == "bf16" else self._NF4_KINDS if frozen_weights == "nf4" else tuple(frozen_weights)
-        if isinstance(frozen_weights, str) and frozen_weights not in ("bf16", "nf4") or not set(kinds) <= set(self._NF4_KINDS):
-            raise lib.QfxError(f"frozen_weights={frozen_weights!r}: 'bf16', 'nf4' or a subset of {self._NF4_KINDS}")
+        kinds = () if frozen_weights in ("bf16", "fp8") else self._NF4_KINDS if frozen_weights == "nf4" else tuple(frozen_weights)
+        if isinstance(frozen_weights, str) and frozen_weights not in ("bf16", "nf4", "fp8") or not set(kinds) <= set(self._NF4_KINDS):
+            raise lib.QfxError(f"frozen_weights={frozen_weights!r}: 'bf16', 'nf4', 'fp8' or a subset of {self._NF4_KINDS}")
         self._nf4_kinds, self.nf4_blocksize = tuple(k for k in self._NF4_KINDS if k in kinds), int(nf4_blocksize)
         self._nf4_store = {}     # NF4-resident kind -> (codes uint8 [L, ..., in/2], absmax fp32 [L, n/blocksize])
         self._nf4_rings = None   # sharding.Nf4Blocks of (double, single) blocks
-        self._blk_rings = None   # (double, single) rings the block weights come through: NF4 dequantization or sharding
+        self._fp8_kinds = self._NF4_KINDS if frozen_weights == "fp8" else ()
+        self._fp8_store = {}     # FP8-resident kind -> codes float8_e4m3fn [L, ..., out, in]
+        self._expand_rings = None  # sharding.Nf4Blocks / Fp8Blocks of (double, single) blocks: filled from resident storage
+        self._blk_rings = None   # (double, single) rings the block weights come through: NF4 / FP8 expansion or sharding
         self.dev = torch.device(device)
         self.sites = {}          # (l, grp, s) -> LoraSite   (l = -1: input embedders)
         self.mod_sites = {}      # kind -> dict(idx=[row indices], names=[...], A=[n, r, D], B=[n, C, r], ga, gb)  (AdaLN linears)
@@ -218,8 +225,12 @@ class FusedMMDiTBase(nn.Module):
         self._fwd_gen = 0        # bumped by every forward: autograd nodes of an older forward refuse to run (their activations are gone)
 
     def _frozen(self, kind, *shape):
-        """A stacked block matrix [L, ..., out, in]: bf16 zeros, or — NF4-resident — its codes and absmax (in `self._nf4_store`; the
-        bf16 stack is never allocated and `self.w[kind]` becomes a ring view in `_finish_frozen`)."""
+        """A stacked block matrix [L, ..., out, in]: bf16 zeros, or — NF4-resident — its codes and absmax (in `self._nf4_store`), or
+        — FP8-resident — its e4m3fn codes (in `self._fp8_store`).  A resident kind's bf16 stack is never allocated and `self.w[kind]`
+        becomes a ring view in `_finish_frozen`."""
+        if kind in self._fp8_kinds:
+            self._fp8_store[kind] = torch.zeros(*shape, device=self.dev, dtype=torch.uint8).view(torch.float8_e4m3fn)
+            return None
         if kind not in self._nf4_kinds:
             return torch.zeros(*shape, device=self.dev, dtype=BF)
         if shape[-1] % self.nf4_blocksize:
@@ -230,23 +241,31 @@ class FusedMMDiTBase(nn.Module):
         return None
 
     def _finish_frozen(self):
-        """NF4-resident kinds: one two-slot ring per block kind, filled by dequantizing a block right before it runs."""
-        if not self._nf4_kinds:
+        """NF4- or FP8-resident kinds: one two-slot ring per block kind, filled by dequantizing (NF4) or expanding (FP8) a block
+        right before it runs."""
+        if not (self._nf4_kinds or self._fp8_kinds):
             return
-        from .sharding import Nf4Blocks
+        from .sharding import Fp8Blocks, Nf4Blocks
         rings = []
         for per, n in ((self._PER_LAYER, self.L), (self._PER_SINGLE, self.Ls)):
-            st = {k: (*self._nf4_store[k], tuple(self._nf4_store[k][0].shape[1:-1]) + (self._nf4_store[k][0].shape[-1] * 2,))
-                  for k in per if k in self._nf4_store}
-            rings.append(Nf4Blocks(st, n, self.nf4_blocksize) if st else None)
+            if self._fp8_kinds:
+                st = {k: self._fp8_store[k] for k in per if k in self._fp8_store}
+                rings.append(Fp8Blocks(st, n) if st else None)
+            else:
+                st = {k: (*self._nf4_store[k], tuple(self._nf4_store[k][0].shape[1:-1]) + (self._nf4_store[k][0].shape[-1] * 2,))
+                      for k in per if k in self._nf4_store}
+                rings.append(Nf4Blocks(st, n, self.nf4_blocksize) if st else None)
             for k in st:
                 self.w[k] = rings[-1].rings[k]
-        self._nf4_rings = self._blk_rings = tuple(rings)
+        self._expand_rings = self._blk_rings = tuple(rings)
+        if self._nf4_kinds:
+            self._nf4_rings = self._expand_rings
 
     @property
     def frozen_weights(self) -> str:
-        """How the frozen block weights are stored: "bf16", or "nf4" (NF4-resident, dequantized block by block)."""
-        return "nf4" if self._nf4_kinds else "bf16"
+        """How the frozen block weights are stored: "bf16", "nf4" (NF4-resident, dequantized block by block) or "fp8"
+        (float8-e4m3fn-resident, expanded block by block)."""
+        return "fp8" if self._fp8_kinds else "nf4" if self._nf4_kinds else "bf16"
 
     @property
     def device(self):
@@ -268,6 +287,9 @@ class FusedMMDiTBase(nn.Module):
         if self._nf4_kinds:
             raise lib.QfxError("shard_frozen_weights: the frozen weights are NF4-resident (frozen_weights='nf4'); sharded NF4 is not "
                                "supported — shard a bf16 model or train the NF4 model on one GPU per replica")
+        if self._fp8_kinds:
+            raise lib.QfxError("shard_frozen_weights: the frozen weights are FP8-resident (frozen_weights='fp8'); sharded FP8 is not "
+                               "supported — shard a bf16 model or train the FP8 model on one GPU per replica")
         self._sharded = ShardedBlocks({k: self.w[k] for k in self._PER_LAYER}, self.L, group, gather=gather)
         for k in self._PER_LAYER:
             self.w[k] = self._sharded.rings[k]
@@ -299,8 +321,8 @@ class FusedMMDiTBase(nn.Module):
         if ring is not None:
             ring.release(l)
 
-    def _join_nf4_rings(self):
-        for ring in self._nf4_rings or ():
+    def _join_expand_rings(self):
+        for ring in self._expand_rings or ():
             if ring is not None:
                 ring.join()
 
@@ -369,9 +391,12 @@ class FusedMMDiTBase(nn.Module):
     def load_state_dict(self, sd, strict=True, assign=False):
         """bf16 checkpoints, and 4-bit NF4 base checkpoints (bitsandbytes `Linear4bit` entries, nf4.py): NF4 block matrices go to the
         NF4-resident storage of a model constructed with frozen_weights='nf4' (`from_reference` does), NF4 tensors outside the blocks
-        are dequantized to bf16 here."""
+        are dequantized to bf16 here.  Into a model constructed with frozen_weights='fp8': block matrices as float8_e4m3fn or as their
+        exact bf16 upcast (fp8.py).  A float8 tensor anywhere else, or into a bf16 model, is upcast to bf16."""
         from . import nf4
         plain, quant = nf4.split_state_dict(sd)
+        if self._fp8_kinds:
+            return self._load_fp8(plain, quant, strict)
         if quant or self._nf4_kinds:
             return self._load_nf4(plain, quant, strict)
         views = self._weight_views()
@@ -440,6 +465,49 @@ class FusedMMDiTBase(nn.Module):
                 codes.view(-1)[o // 2:(o + n) // 2].copy_(q.codes.to(self.dev))
                 absmax.view(-1)[o // q.blocksize:(o + n) // q.blocksize].copy_(q.absmax.to(self.dev))
             seen.add(kk)
+        missing = [k for k in list(views) + list(self._lora_params) if k not in seen]
+        if strict and (unexpected or [m for m in missing if "lora" not in m]):
+            raise KeyError(f"load_state_dict: missing {missing[:5]}..., unexpected {unexpected[:5]}...")
+        return missing, unexpected
+
+    def _load_fp8(self, plain, quant, strict):
+        """load_state_dict into an FP8-resident model: a block matrix goes to the e4m3fn stack of its kind (a meta view's storage
+        offset locates its elements), after fp8.as_e4m3 has checked it; every other entry loads as into a bf16 model."""
+        from . import fp8
+        if quant:
+            raise lib.QfxError(f"`{next(iter(quant))}` is a bitsandbytes NF4 weight, but this model keeps its block matrices FP8-resident "
+                               f"(frozen_weights='fp8'): construct it with frozen_weights='nf4' (from_reference does) for a 4-bit base "
+                               f"checkpoint")
+        views = self._weight_views(store=True)
+        unexpected, seen, form = [], set(), {}
+
+        def canon(k):
+            k = k.replace(".base_layer.", ".")
+            return k[len("transformer."):] if k.startswith("transformer.") and k[len("transformer."):] in views else k
+
+        for k, v in plain.items():
+            kk, lk = canon(k), self._canonical_lora_key(k)
+            if kk in views:
+                t = views[kk]
+                if t.is_meta:
+                    kind = self._matrix_kind(kk)
+                    first = form.setdefault(kind, (v.dtype, kk))
+                    if v.dtype != first[0]:
+                        raise lib.QfxError(f"`{kk}` arrives as {v.dtype}, but `{first[1]}` of the same stacked kind {kind} arrived as "
+                                           f"{first[0]}: the layers of a stacked kind must arrive in one format")
+                    if tuple(v.shape) != tuple(t.shape):
+                        raise lib.QfxError(f"`{kk}`: shape {tuple(v.shape)}, the model expects {tuple(t.shape)}")
+                    o, n = t.storage_offset(), t.numel()
+                    codes = fp8.as_e4m3(kk, v, self.dev)
+                    self._fp8_store[kind].view(torch.uint8).view(-1)[o:o + n].copy_(codes.view(torch.uint8).reshape(-1))
+                else:
+                    t.copy_(v.to(self.dev, BF))
+                seen.add(kk)
+            elif lk in self._lora_params:
+                self._lora_params[lk].copy_(v.to(self.dev, BF))
+                seen.add(lk)
+            else:
+                unexpected.append(k)
         missing = [k for k in list(views) + list(self._lora_params) if k not in seen]
         if strict and (unexpected or [m for m in missing if "lora" not in m]):
             raise KeyError(f"load_state_dict: missing {missing[:5]}..., unexpected {unexpected[:5]}...")
@@ -621,6 +689,9 @@ class FusedMMDiTBase(nn.Module):
             raise lib.QfxError("merge_adapter: the frozen weights are sharded; merge on a replicated model")
         if self._nf4_kinds:
             raise lib.QfxError("merge_adapter: the frozen weights are NF4-resident (frozen_weights='nf4'); merge on a bf16 model")
+        if self._fp8_kinds:
+            raise lib.QfxError("merge_adapter: the frozen weights are FP8-resident (frozen_weights='fp8'): W + scaling * B A is not an "
+                               "e4m3fn value; merge on a bf16 model")
         if not self._lora_params or getattr(self, "_merged", None):
             return
         views, parked = self._weight_views(), {}
@@ -1134,7 +1205,7 @@ class FusedMMDiTBase(nn.Module):
         D, L, Mt, w, sh = self.D, self.L, ws["Mt"], self.w, self._blk_rings
         nb = L + self.Ls
         xi = lambda i: ws["X"][i] if train else ws["X"][i & 1]
-        for ring in self._nf4_rings or ():  # every forward fills the same blocks: eager, captured and replayed alike
+        for ring in self._expand_rings or ():  # every forward fills the same blocks: eager, captured and replayed alike
             if ring is not None:
                 ring.reset()
         for blk in range(nb):
@@ -1147,7 +1218,7 @@ class FusedMMDiTBase(nn.Module):
                 self._single_fwd(ws, blk - L, xi(blk), xi(blk + 1), ws["sgl"][(blk - L) if train else 0])
             if sh is not None:
                 self._release(blk)
-        self._join_nf4_rings()
+        self._join_expand_rings()
         Xl = ws["Xlast"] = xi(nb)
         lib.ln_modulate_fwd(Xl[Mt:], ws["hn"], ws["fmod"][:, D:], ws["fmod"][:, :D], ws["Limg"], ws["fstats"][0], ws["fstats"][1])
         lib.gemm([lib.gemm_problem(ws["hn"], w["proj_out_w"], ws["pred"], bias=w["proj_out_b"])], self.C_out, D)
@@ -1185,7 +1256,7 @@ class FusedMMDiTBase(nn.Module):
             if self._blk_rings is not None:
                 self._release(blk)
             dX = dXn
-        self._join_nf4_rings()
+        self._join_expand_rings()
         self._mod_lora_bwd(ws)
         for key, s, _ in self._embed_table().values():
             self._embed_bwd(ws, key, s, dX)

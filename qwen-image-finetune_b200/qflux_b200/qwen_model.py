@@ -80,7 +80,9 @@ class QwenImageB200(FusedMMDiTBase):
     def __init__(self, cfg: QwenB200Config, device="cuda", _host_only: bool = False, frozen_weights="bf16", nf4_blocksize: int = 64):
         """`_host_only=True` (tests of the naming / LoRA-registry logic) allocates on `device` without requiring CUDA;
         every compute entry point still raises on non-CUDA tensors.  frozen_weights="nf4": the block matrices of a 4-bit base
-        checkpoint stay NF4-resident (codes + fp32 absmax per `nf4_blocksize` elements) and are dequantized block by block."""
+        checkpoint stay NF4-resident (codes + fp32 absmax per `nf4_blocksize` elements) and are dequantized block by block;
+        frozen_weights="fp8": the block matrices of a float8-e4m3fn checkpoint stay FP8-resident (one byte per element) and are
+        expanded to bf16 block by block."""
         super().__init__()
         self._init_common(device, _host_only, frozen_weights, nf4_blocksize)
         assert cfg.attention_head_dim == 128, "the sm_90a attention kernels are specialised for head_dim 128"

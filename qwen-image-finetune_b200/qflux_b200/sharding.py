@@ -17,8 +17,9 @@ parallel mode.  B200-first layout instead of FSDP's per-module flat parameters:
     for another.  `gather="nccl"` (or QFX_SHARD_GATHER=nccl, or ranks on different hosts) keeps the all_gather_into_tensor path;
   * kernels keep reading plain row-major [out, in] views — the views now point into the gather buffer of the block's slot.
 
-The same two-slot ring (`BlockRing`) has a second fill source: `Nf4Blocks` dequantizes a block's NF4-resident matrices
-(4-bit base checkpoints, nf4.py) into its slot with one kernel launch.
+The same two-slot ring (`BlockRing`) has two more fill sources: `Nf4Blocks` dequantizes a block's NF4-resident matrices
+(4-bit base checkpoints, nf4.py) into its slot with one kernel launch, and `Fp8Blocks` expands its FP8-resident matrices
+(float8-e4m3fn base checkpoints, fp8.py) the same way.
 """
 from __future__ import annotations
 
@@ -52,7 +53,7 @@ class LayerRing:
 class BlockRing:
     """Two-slot ring of one block kind's weights: block l is filled into slot l & 1 on a side stream (`prefetch`), kernels on
     the compute stream wait for it (`acquire`), and the slot is refilled only after its last reader has finished (`release`).
-    Subclasses provide the fill source (`_fill(slot, l)`): an all-gather of the ranks' shards, or the NF4 dequantization."""
+    Subclasses provide the fill source (`_fill(slot, l)`): an all-gather of the ranks' shards, the NF4 dequantization or the FP8 expansion."""
 
     def _layout(self, shapes: dict, n_layers: int, dev, dtype) -> int:
         """One LayerRing view per tensor, each starting on an ALIGN boundary of the slot.  Returns the elements a slot needs."""
@@ -233,3 +234,21 @@ class Nf4Blocks(BlockRing):
         from . import lib
         lib.nf4_dequant([(c[l].reshape(-1), a[l].reshape(-1), self.gbuf[s, self.rings[k].offset: self.rings[k].offset + self.rings[k].numel],
                           self.blocksize) for k, (c, a, _) in self.stacks.items()])
+
+
+class Fp8Blocks(BlockRing):
+    """FP8-resident frozen weights: every FP8 matrix of a block kind lives as layer-stacked float8-e4m3fn codes (fp8.py), one byte
+    per element in the bf16 layout; a block's bf16 matrices are produced in its ring slot by ONE qfx_fp8_expand launch right before
+    it runs (exact: every finite e4m3fn value is a bf16 value)."""
+
+    def __init__(self, stacks: dict, n_layers: int):
+        """stacks: {name: codes float8_e4m3fn [L, ...] (the bf16 shape of the stack)}."""
+        codes0 = next(iter(stacks.values()))
+        off = self._layout({k: tuple(c.shape[1:]) for k, c in stacks.items()}, n_layers, codes0.device, torch.bfloat16)
+        self.stacks = stacks
+        self._alloc_slots(off)
+
+    def _fill(self, s: int, l: int):
+        from . import lib
+        lib.fp8_expand([(c[l].reshape(-1), self.gbuf[s, self.rings[k].offset: self.rings[k].offset + self.rings[k].numel])
+                        for k, c in self.stacks.items()])
