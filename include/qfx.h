@@ -214,6 +214,48 @@ int qfx_fused_adamw(const qfx_adamw_tensor* tensors, const int* chunks, int n_ch
                     float beta2, float eps, float weight_decay, int step, void* stream);
 
 /* ------------------------------------------------------------------------------------------------------------------
+ * Deterministic variants (selected by the host when torch.use_deterministic_algorithms(True) is in effect).  Each computes what
+ * the entry point it is named after computes, with the same arguments and accumulate / overwrite contract, but without
+ * floating-point atomics: every cross-CTA sum is formed in a fixed order, so two calls on the same inputs give the same bits on
+ * the same GPU.  Reductions store per-CTA partials with plain stores into caller-owned fp32 `scratch` (nothing is allocated
+ * inside a call) and a second launch adds them up in split order.  Split counts depend on the shapes only, never on the SM count;
+ * each function refuses a scratch smaller than its rule below, before any CUDA call.
+ *
+ * qfx_attn_bwd_det: dQ, dK, dV of qfx_attn_bwd.  dK / dV come from qfx_attn_bwd's key-major kernel without its dQ phase; dQ from a
+ *   query-major kernel (one CTA per 128-query tile, looping over the 64-key tiles in ascending order) that adds every element of
+ *   dQ_accum once.  Rows >= kv_len[b] of dQ_accum are left untouched.  No scratch. */
+int qfx_attn_bwd_det(const void* Q, const void* K, const void* V, const void* dO, const float* lse, const float* delta,
+                     float* dQ_accum, void* dK, void* dV, const int* kv_len, const int* txt_len, int split, int B, int H, int S,
+                     float softmax_scale, void* stream);
+/* qfx_lora_wgrad_tc_det: qfx_lora_wgrad_tc.  With NG = (mode == 1 ? 1 : G) and tiles = Na / 128:
+ *   splits = max(1, min(ceil(M / 256), ceil(QFX_DET_WGRAD_CTAS / tiles))),  rows = 64 * ceil(ceil(M / splits) / 64),
+ *   scratch_floats >= ceil(M / rows) * Na * NG * r            (at most ~QFX_DET_WGRAD_CTAS partial tiles of 128 x NG*r). */
+#define QFX_DET_WGRAD_CTAS 264
+int qfx_lora_wgrad_tc_det(const void* A, int64_t lda, int Na, const void* B, int64_t ldb, int G, int M, int mode, int Dg,
+                          float* const* Gp, int64_t gs_i, int64_t gs_j, int r, float* scratch, int64_t scratch_floats, void* stream);
+/* qfx_lora_wgrad_det: qfx_lora_wgrad (r in 4/8/16/32/64).  rows = 64 * ceil(ceil(M / ceil(M / 512)) / 64),
+ *   scratch_floats >= ceil(M / rows) * Dp * r. */
+int qfx_lora_wgrad_det(const void* P, int64_t ldp, const void* Q, int64_t ldq, float* G, int64_t gs_i, int64_t gs_j, int M, int Dp,
+                       int r, float* scratch, int64_t scratch_floats, void* stream);
+/* qfx_mod_grad_det: qfx_mod_grad.  With B = M / rows_per_batch and cb = ceil(D / 256):
+ *   splits = max(1, min(ceil(rows_per_batch / 32), ceil(QFX_DET_MODGRAD_CTAS / (cb * B)))),  scratch_floats >= splits * 2 * B * D. */
+#define QFX_DET_MODGRAD_CTAS 528
+int qfx_mod_grad_det(const void* g, int64_t ldg, const void* m, int64_t ldm, const float* mean, const float* rstd, int rows_per_batch,
+                     float* sum_out, float* prod_out, int64_t ldo, int M, int D, float* scratch, int64_t scratch_floats, void* stream);
+/* qfx_flow_loss_det: qfx_flow_loss (loss is overwritten).  scratch_floats >= QFX_DET_LOSS_PARTIALS. */
+#define QFX_DET_LOSS_PARTIALS 296
+int qfx_flow_loss_det(const void* pred, const void* x0, const void* noise, const float* w, float norm, float grad_scale, float* loss,
+                      void* dpred, int B, int L, int Ltot, int C, float* scratch, int64_t scratch_floats, void* stream);
+/* qfx_grad_finalize_det / qfx_fused_adamw_det: the gradient norm behind the clip of qfx_grad_finalize / qfx_fused_adamw.
+ *   scratch_floats >= QFX_DET_NORM_PARTIALS. */
+#define QFX_DET_NORM_PARTIALS 592
+int qfx_grad_finalize_det(const float* g, int64_t n, float pre_scale, float max_norm, float* sumsq, void* out_bf16, float* scratch,
+                          int64_t scratch_floats, void* stream);
+int qfx_fused_adamw_det(const qfx_adamw_tensor* tensors, const int* chunks, int n_chunks, const float* grad, int64_t n_grad,
+                        float* exp_avg, float* exp_avg_sq, float* sumsq, float pre_scale, float max_norm, float lr, float beta1,
+                        float beta2, float eps, float weight_decay, int step, float* scratch, int64_t scratch_floats, void* stream);
+
+/* ------------------------------------------------------------------------------------------------------------------
  * NF4 frozen weights (4-bit base checkpoints: bitsandbytes `Linear4bit`, whose forward dequantizes the weight to bf16 and runs a
  * plain matmul, bitsandbytes/functional.py dequantize_4bit).  One launch dequantizes up to QFX_NF4_MAX_SEGMENTS tensors (the NF4
  * matrices of one block) into bf16:  out[i] = bf16_rn(NF4[nibble_i] * absmax[i / blocksize])  with the product in fp32,

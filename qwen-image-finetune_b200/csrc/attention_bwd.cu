@@ -49,6 +49,8 @@ __device__ __forceinline__ uint32_t mul_bf16x2(uint32_t a, uint32_t b) {
   return r;
 }
 
+// kDQ = false: dK and dV only (the deterministic backward; its dQ comes from attn_bwd_dq_kernel below).
+template <bool kDQ = true>
 __global__ void __launch_bounds__(256, 1) attn_bwd_kernel(const __grid_constant__ AttnBwdParams P) {
   extern __shared__ uint8_t smem_raw[];
   const uint32_t smem_base = (smem_u32(smem_raw) + 1023u) & ~1023u;
@@ -154,16 +156,18 @@ __global__ void __launch_bounds__(256, 1) attn_bwd_kernel(const __grid_constant_
           da[2 * jj + hh] = d;
         }
       }
-      // dS^T to shared memory: [128 keys][64 queries], 128B-swizzled rows (the MN-major A operand of dQ)
+      if constexpr (kDQ) {
+        // dS^T to shared memory: [128 keys][64 queries], 128B-swizzled rows (the MN-major A operand of dQ)
 #pragma unroll
-      for (int jj = 0; jj < 8; ++jj)
+        for (int jj = 0; jj < 8; ++jj)
 #pragma unroll
-        for (int hh = 0; hh < 2; ++hh) {
-          const int kr = cw * 64 + 16 * w + (l >> 2) + 8 * hh;
-          const uint32_t addr = sdS + kr * 128 + ((uint32_t)(jj ^ (kr & 7)) << 4) + (l & 3) * 4;
-          asm volatile("st.shared.b32 [%0], %1;" ::"r"(addr), "r"(da[2 * jj + hh]) : "memory");
-        }
-      fence_proxy_async_smem();
+          for (int hh = 0; hh < 2; ++hh) {
+            const int kr = cw * 64 + 16 * w + (l >> 2) + 8 * hh;
+            const uint32_t addr = sdS + kr * 128 + ((uint32_t)(jj ^ (kr & 7)) << 4) + (l & 3) * 4;
+            asm volatile("st.shared.b32 [%0], %1;" ::"r"(addr), "r"(da[2 * jj + hh]) : "memory");
+          }
+        fence_proxy_async_smem();
+      }
       // A fragment of k-chunk c (queries 16 c ..): {pair(jj = 2c, h 0), pair(2c, h 1), pair(2c + 1, h 0), pair(2c + 1, h 1)}
       reg_fence(dv, 64);
       reg_fence(dk, 64);
@@ -173,27 +177,33 @@ __global__ void __launch_bounds__(256, 1) attn_bwd_kernel(const __grid_constant_
 #pragma unroll
       for (int c = 0; c < 4; ++c) wgmma_rs_n128<1>(dk, da + 4 * c, sdesc_sw128(sQ(st) + c * 2048, BW_Q_ATOM, 1024), 1);
       wgmma_commit();
-      named_bar(1, 256);  // dS^T of both warpgroups is in shared memory
-      float dq[32];
-      reg_fence(dq, 32);
-      wgmma_fence();
+      if constexpr (kDQ) {
+        named_bar(1, 256);  // dS^T of both warpgroups is in shared memory
+        float dq[32];
+        reg_fence(dq, 32);
+        wgmma_fence();
 #pragma unroll
-      for (int c = 0; c < 8; ++c)
-        wgmma_ss_n64<1, 1>(dq, sdesc_sw128(sdS + c * 2048, BW_Q_ATOM, 1024), sdesc_sw128(sK + cw * BW_KV_ATOM + c * 2048, BW_KV_ATOM, 1024),
-                           c != 0);
-      wgmma_commit();
-      wgmma_wait<0>();
-      reg_fence(dq, 32);
-      reg_fence(dv, 64);
-      reg_fence(dk, 64);
+        for (int c = 0; c < 8; ++c)
+          wgmma_ss_n64<1, 1>(dq, sdesc_sw128(sdS + c * 2048, BW_Q_ATOM, 1024), sdesc_sw128(sK + cw * BW_KV_ATOM + c * 2048, BW_KV_ATOM, 1024),
+                             c != 0);
+        wgmma_commit();
+        wgmma_wait<0>();
+        reg_fence(dq, 32);
+        reg_fence(dv, 64);
+        reg_fence(dk, 64);
 #pragma unroll
-      for (int hh = 0; hh < 2; ++hh) {
-        const int q = q0 + 16 * w + (l >> 2) + 8 * hh;
-        if (q < P.S) {
-          float* dst = P.dQ + ((int64_t)bh * P.S + q) * 128 + cw * 64 + 2 * (l & 3);
+        for (int hh = 0; hh < 2; ++hh) {
+          const int q = q0 + 16 * w + (l >> 2) + 8 * hh;
+          if (q < P.S) {
+            float* dst = P.dQ + ((int64_t)bh * P.S + q) * 128 + cw * 64 + 2 * (l & 3);
 #pragma unroll
-          for (int jj = 0; jj < 8; ++jj) red_add_v2(dst + 8 * jj, dq[4 * jj + 2 * hh], dq[4 * jj + 2 * hh + 1]);
+            for (int jj = 0; jj < 8; ++jj) red_add_v2(dst + 8 * jj, dq[4 * jj + 2 * hh], dq[4 * jj + 2 * hh + 1]);
+          }
         }
+      } else {
+        wgmma_wait<0>();
+        reg_fence(dv, 64);
+        reg_fence(dk, 64);
       }
       named_bar(1, 256);  // stage st and the dS^T buffer are free
       if (threadIdx.x == 0 && i + 2 < n_q) load_q(i + 2);
@@ -210,6 +220,144 @@ __global__ void __launch_bounds__(256, 1) attn_bwd_kernel(const __grid_constant_
     for (int jj = 0; jj < 16; ++jj) {
       *reinterpret_cast<uint32_t*>(dK + 8 * jj) = pack_bf16(dk[4 * jj + 2 * hh], dk[4 * jj + 2 * hh + 1]);
       *reinterpret_cast<uint32_t*>(dV + 8 * jj) = pack_bf16(dv[4 * jj + 2 * hh], dv[4 * jj + 2 * hh + 1]);
+    }
+  }
+}
+
+// Deterministic dQ: query-major, one CTA per (128-query tile, batch*head), two warpgroups of 64 query rows each; thread 0 issues
+// the TMA loads (Q and dO once, a two-stage ring of 64-key tiles of K and V).  Per key tile j the scores are recomputed:
+//     S   = Q K_j^T            wgmma SS   A = Q  (K-major)     B = K_j (K-major)
+//     dP  = dO V_j^T           wgmma SS   A = dO (K-major)     B = V_j (K-major)
+//     P   = exp2(S c - L_q) ;  dS = P o (dP - delta_q) * scale     (registers; the same bf16 rounding points as attn_bwd_kernel)
+//     dQ += dS K_j             wgmma RS   A = dS from registers     B = K_j read MN-major
+// over the key tiles in ascending order, so every dQ element is one register sum in a fixed order, added ONCE to the caller's buffer.
+// 64-key tiles keep the three accumulators (S, dP: 32 registers each, dQ: 64) well inside the register file.
+constexpr int DQ_KT = 64 * 128 * 2;     // 16 KB: K_j or V_j tile, two atoms of 8 KB
+constexpr int DQ_KT_ATOM = 64 * 128;
+constexpr int DQ_QT = 128 * 128 * 2;    // 32 KB: Q or dO tile, two atoms of 16 KB
+constexpr int DQ_QT_ATOM = 128 * 128;
+constexpr int DQ_SMEM = 2 * DQ_QT + 4 * DQ_KT + 1024 /*align slack*/ + 256;
+
+__global__ void __launch_bounds__(256, 1) attn_bwd_dq_kernel(const __grid_constant__ AttnBwdParams P) {
+  extern __shared__ uint8_t smem_raw[];
+  const uint32_t smem_base = (smem_u32(smem_raw) + 1023u) & ~1023u;
+  const uint32_t sQ = smem_base, sdO = smem_base + DQ_QT;
+  auto sK = [&](int st) { return smem_base + 2 * DQ_QT + st * DQ_KT; };
+  auto sV = [&](int st) { return smem_base + 2 * DQ_QT + (2 + st) * DQ_KT; };
+  const uint32_t bar_base = smem_base + 2 * DQ_QT + 4 * DQ_KT;
+  const uint32_t q_full = bar_base;
+  auto kv_full = [&](int st) { return bar_base + 8u * (1 + st); };
+
+  const int q0 = blockIdx.x * 128;
+  const int bh = blockIdx.y;
+  const int b = bh / P.H;
+  const int kv_len = min(P.kv_len ? P.kv_len[b] : P.S, P.S);
+  const int txt_len = P.txt_len ? P.txt_len[b] : P.split;
+  // query tiles of only padding rows (>= kv_len[b]) add nothing; key tiles wholly inside the text padding [txt_len, split) are
+  // skipped: the live tiles are [0, n_txt) and [img0, n_k)
+  const int n_k = (kv_len + 63) / 64;
+  const int n_txt = min((txt_len + 63) / 64, n_k);
+  const int img0 = max(P.split / 64, n_txt);
+  const int n_live = n_txt + max(0, n_k - img0);
+  if (q0 >= kv_len || n_live == 0) return;
+  auto tile = [&](int i) { return i < n_txt ? i : img0 + (i - n_txt); };
+
+  if (threadIdx.x == 0) {
+    mbar_init(q_full, 1);
+    mbar_init(kv_full(0), 1);
+    mbar_init(kv_full(1), 1);
+    fence_barrier_init();
+  }
+  __syncthreads();
+  auto load_kv = [&](int i) {
+    const int st = i & 1, k0 = tile(i) * 64;
+    mbar_expect_tx(kv_full(st), 2 * DQ_KT);
+    tma_load_3d(sK(st), &P.tmK, kv_full(st), 0, k0, bh);
+    tma_load_3d(sK(st) + DQ_KT_ATOM, &P.tmK, kv_full(st), 64, k0, bh);
+    tma_load_3d(sV(st), &P.tmV, kv_full(st), 0, k0, bh);
+    tma_load_3d(sV(st) + DQ_KT_ATOM, &P.tmV, kv_full(st), 64, k0, bh);
+  };
+  if (threadIdx.x == 0) {
+    mbar_expect_tx(q_full, 2 * DQ_QT);
+    tma_load_3d(sQ, &P.tmQ, q_full, 0, q0, bh);
+    tma_load_3d(sQ + DQ_QT_ATOM, &P.tmQ, q_full, 64, q0, bh);
+    tma_load_3d(sdO, &P.tmdO, q_full, 0, q0, bh);
+    tma_load_3d(sdO + DQ_QT_ATOM, &P.tmdO, q_full, 64, q0, bh);
+    load_kv(0);
+    if (n_live > 1) load_kv(1);
+  }
+
+  const int cw = threadIdx.x >> 7;
+  const int t = threadIdx.x & 127, w = t >> 5, l = t & 31;
+  float L[2], D[2];
+#pragma unroll
+  for (int hh = 0; hh < 2; ++hh) {
+    const int q = q0 + cw * 64 + 16 * w + (l >> 2) + 8 * hh;
+    L[hh] = q < P.S ? P.lse[(int64_t)bh * P.S + q] : INFINITY;  // queries past S: P = 0
+    D[hh] = q < P.S ? P.delta[(int64_t)bh * P.S + q] * P.scale : 0.f;
+  }
+  float dq[64];
+#pragma unroll
+  for (int e = 0; e < 64; ++e) dq[e] = 0.f;
+  const uint32_t aQ = sQ + cw * 64 * 128, adO = sdO + cw * 64 * 128;
+  mbar_wait(q_full, 0);
+  for (int i = 0; i < n_live; ++i) {
+    const int st = i & 1, k0 = tile(i) * 64;
+    float sc[32], dp[32];
+    mbar_wait(kv_full(st), (i >> 1) & 1);
+    reg_fence(sc, 32);
+    reg_fence(dp, 32);
+    wgmma_fence();
+#pragma unroll
+    for (int k = 0; k < 8; ++k)
+      wgmma_ss_n64<0, 0>(sc, sdesc_sw128(aQ + (k >> 2) * DQ_QT_ATOM + (k & 3) * 32, 16, 1024),
+                         sdesc_sw128(sK(st) + (k >> 2) * DQ_KT_ATOM + (k & 3) * 32, 16, 1024), k != 0);
+#pragma unroll
+    for (int k = 0; k < 8; ++k)
+      wgmma_ss_n64<0, 0>(dp, sdesc_sw128(adO + (k >> 2) * DQ_QT_ATOM + (k & 3) * 32, 16, 1024),
+                         sdesc_sw128(sV(st) + (k >> 2) * DQ_KT_ATOM + (k & 3) * 32, 16, 1024), k != 0);
+    wgmma_commit();
+    wgmma_wait<0>();
+    reg_fence(sc, 32);
+    reg_fence(dp, 32);
+    // keys >= kv_len[b] and the text padding [txt_len[b], split) get P = 0 (only tiles that contain such keys pay for the test)
+    const bool partial = k0 + 64 > kv_len || (txt_len < P.split && k0 < P.split && k0 + 64 > txt_len);
+    uint32_t da[16];
+#pragma unroll
+    for (int jj = 0; jj < 8; ++jj)
+#pragma unroll
+      for (int hh = 0; hh < 2; ++hh) {
+        const int r = 4 * jj + 2 * hh;
+        float p0 = exp2f(sc[r] * P.scale_log2 - L[hh]), p1 = exp2f(sc[r + 1] * P.scale_log2 - L[hh]);
+        if (partial) {
+          const int key = k0 + 8 * jj + 2 * (l & 3);
+          if (key >= kv_len || (key >= txt_len && key < P.split)) p0 = 0.f;
+          if (key + 1 >= kv_len || (key + 1 >= txt_len && key + 1 < P.split)) p1 = 0.f;
+        }
+        da[2 * jj + hh] = mul_bf16x2(pack_bf16(p0, p1), pack_bf16(dp[r] * P.scale - D[hh], dp[r + 1] * P.scale - D[hh]));
+      }
+    reg_fence(dq, 64);
+    wgmma_fence();
+#pragma unroll
+    for (int c = 0; c < 4; ++c) wgmma_rs_n128<1>(dq, da + 4 * c, sdesc_sw128(sK(st) + c * 2048, DQ_KT_ATOM, 1024), 1);
+    wgmma_commit();
+    wgmma_wait<0>();
+    reg_fence(dq, 64);
+    named_bar(1, 256);  // both warpgroups are done with stage st
+    if (threadIdx.x == 0 && i + 2 < n_live) load_kv(i + 2);
+  }
+  // epilogue: one read-modify-write per element of the rows < kv_len[b]
+#pragma unroll
+  for (int hh = 0; hh < 2; ++hh) {
+    const int q = q0 + cw * 64 + 16 * w + (l >> 2) + 8 * hh;
+    if (q >= kv_len) continue;
+    float2* dst = reinterpret_cast<float2*>(P.dQ + ((int64_t)bh * P.S + q) * 128 + 2 * (l & 3));
+#pragma unroll
+    for (int jj = 0; jj < 16; ++jj) {
+      float2 v = dst[4 * jj];
+      v.x += dq[4 * jj + 2 * hh];
+      v.y += dq[4 * jj + 2 * hh + 1];
+      dst[4 * jj] = v;
     }
   }
 }
@@ -250,11 +398,53 @@ extern "C" int qfx_attn_bwd(const void* Q, const void* K, const void* V, const v
   P.scale_log2 = softmax_scale * 1.4426950408889634f;
   static bool attr_done = false;
   if (!attr_done) {
-    QFX_CUDA(cudaFuncSetAttribute(attn_bwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, BW_SMEM));
+    QFX_CUDA(cudaFuncSetAttribute(attn_bwd_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, BW_SMEM));
     attr_done = true;
   }
   dim3 grid((S + 127) / 128, B * H);
-  attn_bwd_kernel<<<grid, 256, BW_SMEM, (cudaStream_t)stream>>>(P);
+  attn_bwd_kernel<true><<<grid, 256, BW_SMEM, (cudaStream_t)stream>>>(P);
+  QFX_CUDA(cudaGetLastError());
+  return 0;
+}
+
+/* Deterministic variant (see qfx.h): the same arguments and the same dQ_accum contract, but dK / dV come from attn_bwd_kernel<false>
+ * and dQ from attn_bwd_dq_kernel, which adds each element once — no floating-point atomics, bit-reproducible run to run. */
+extern "C" int qfx_attn_bwd_det(const void* Q, const void* K, const void* V, const void* dO, const float* lse, const float* delta,
+                                float* dQ_accum, void* dK, void* dV, const int* kv_len, const int* txt_len, int split, int B, int H,
+                                int S, float softmax_scale, void* stream) {
+  QFX_CHECK_ARG(B > 0 && H > 0 && S > 0 && dQ_accum && dK && dV && lse && delta, "qfx_attn_bwd_det: bad arguments");
+  QFX_CHECK_ARG(!txt_len || (split > 0 && split <= S), "qfx_attn_bwd_det: txt_len needs 0 < split <= S (split=%d S=%d)", split, S);
+  // dQ is read and written as 8-byte pairs, dK / dV are stored as 4-byte pairs
+  QFX_CHECK_ARG(((uintptr_t)dQ_accum & 7) == 0 && ((uintptr_t)dK & 3) == 0 && ((uintptr_t)dV & 3) == 0,
+                "qfx_attn_bwd_det: dQ_accum must be 8-byte aligned, dK / dV 4-byte aligned");
+  AttnBwdParams P, Pq;
+  memset(&P, 0, sizeof(P));
+  memset(&Pq, 0, sizeof(Pq));
+  int rc;
+  if ((rc = make_qkv_tmap(&P.tmK, K, B * H, S))) return rc;
+  if ((rc = make_qkv_tmap(&P.tmV, V, B * H, S))) return rc;
+  if ((rc = make_q64_tmap(&P.tmQ, Q, B * H, S))) return rc;
+  if ((rc = make_q64_tmap(&P.tmdO, dO, B * H, S))) return rc;
+  // the dQ kernel's roles are swapped: 128-row Q / dO tiles, 64-row K / V tiles
+  if ((rc = make_q64_tmap(&Pq.tmK, K, B * H, S))) return rc;
+  if ((rc = make_q64_tmap(&Pq.tmV, V, B * H, S))) return rc;
+  if ((rc = make_qkv_tmap(&Pq.tmQ, Q, B * H, S))) return rc;
+  if ((rc = make_qkv_tmap(&Pq.tmdO, dO, B * H, S))) return rc;
+  P.dQ = dQ_accum; P.dK = (bf16*)dK; P.dV = (bf16*)dV; P.lse = lse; P.delta = delta; P.kv_len = kv_len; P.txt_len = txt_len;
+  P.split = txt_len ? split : 0; P.S = S; P.H = H;
+  P.scale = softmax_scale;
+  P.scale_log2 = softmax_scale * 1.4426950408889634f;
+  Pq.dQ = P.dQ; Pq.lse = lse; Pq.delta = delta; Pq.kv_len = kv_len; Pq.txt_len = txt_len;
+  Pq.split = P.split; Pq.S = S; Pq.H = H; Pq.scale = P.scale; Pq.scale_log2 = P.scale_log2;
+  static bool attr_done = false;
+  if (!attr_done) {
+    QFX_CUDA(cudaFuncSetAttribute(attn_bwd_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, BW_SMEM));
+    QFX_CUDA(cudaFuncSetAttribute(attn_bwd_dq_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, DQ_SMEM));
+    attr_done = true;
+  }
+  attn_bwd_kernel<false><<<dim3((S + 127) / 128, B * H), 256, BW_SMEM, (cudaStream_t)stream>>>(P);
+  QFX_CUDA(cudaGetLastError());
+  attn_bwd_dq_kernel<<<dim3((S + 127) / 128, B * H), 256, DQ_SMEM, (cudaStream_t)stream>>>(Pq);
   QFX_CUDA(cudaGetLastError());
   return 0;
 }

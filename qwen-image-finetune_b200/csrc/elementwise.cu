@@ -201,6 +201,9 @@ __global__ void __launch_bounds__(256) ln_modulate_bwd_kernel(const bf16* __rest
 // Column reductions over the tokens of each sample for the modulation gradients (see qfx_mod_grad in qfx.h).
 // grid (D/256, B, row splits): a CTA owns 256 columns (one uint4 per lane) of one sample's row range, its 8 warps stride over
 // the rows, partials meet in shared memory and leave as one fp32 atomic per column and CTA.
+// kPartial (deterministic variant): sum_out is the split-major partial buffer [splits][2][B][D] (sum, then product) and every CTA
+// stores its column totals there; launch_split_sum adds them up in split order.
+template <bool kPartial = false>
 __global__ void __launch_bounds__(256) mod_grad_kernel(const bf16* __restrict__ g, int64_t ldg, const bf16* __restrict__ m, int64_t ldm,
                                                        const float* __restrict__ mean, const float* __restrict__ rstd,
                                                        int rows_per_batch, float* __restrict__ sum_out, float* __restrict__ prod_out,
@@ -247,8 +250,14 @@ __global__ void __launch_bounds__(256) mod_grad_kernel(const bf16* __restrict__ 
       ts += red[0][w][threadIdx.x];
       tp += red[1][w][threadIdx.x];
     }
-    if (sum_out != nullptr) atomicAdd(sum_out + (int64_t)b * ldo + c, ts);
-    if (prod_out != nullptr && m != nullptr) atomicAdd(prod_out + (int64_t)b * ldo + c, tp);
+    if constexpr (kPartial) {
+      float* part = sum_out + ((int64_t)blockIdx.z * 2 * gridDim.y + b) * D + c;
+      part[0] = ts;
+      part[(int64_t)gridDim.y * D] = tp;
+    } else {
+      if (sum_out != nullptr) atomicAdd(sum_out + (int64_t)b * ldo + c, ts);
+      if (prod_out != nullptr && m != nullptr) atomicAdd(prod_out + (int64_t)b * ldo + c, tp);
+    }
   }
 }
 
@@ -560,6 +569,8 @@ __global__ void flow_noisy_input_var_kernel(const bf16* __restrict__ x0, const b
 
 // loss += norm * sum w[b,t] * (pred - (noise - x0))^2 ;  dpred = 2 * norm * w * (pred - target) * loss_scale  (bf16),
 // zero for the control tokens.  pred is [B, Ltot, C]; only the first L tokens carry loss (trainer :839).
+// kPartial (deterministic variant): loss[blockIdx.x] receives the CTA's share instead of an atomic add.
+template <bool kPartial = false>
 __global__ void __launch_bounds__(256) flow_loss_kernel(const bf16* __restrict__ pred, const bf16* __restrict__ x0,
                                                         const bf16* __restrict__ noise, const float* __restrict__ w,
                                                         float norm, float grad_scale, float* __restrict__ loss,
@@ -588,7 +599,8 @@ __global__ void __launch_bounds__(256) flow_loss_kernel(const bf16* __restrict__
   if (threadIdx.x == 0) {
     float s = 0.f;
     for (int i = 0; i < 8; ++i) s += red[i];
-    atomicAdd(loss, s * norm);
+    if constexpr (kPartial) loss[blockIdx.x] = s * norm;
+    else atomicAdd(loss, s * norm);
   }
 }
 
@@ -596,7 +608,8 @@ __global__ void __launch_bounds__(256) flow_loss_kernel(const bf16* __restrict__
 // G[i, j] += sum_m P[m, i] * Q[m, j]   (i < Dp, j < r <= 64), fp32 atomics into G with strides (gs_i, gs_j) so the same
 // kernel writes dB[out, r] (P = dY, Q = s X A^T) and dA[r, in] (P = X, Q = s dY B; transposed store).
 // Block: 128 columns of P x a chunk of rows; thread = one column i, r fp32 accumulators; Q rows broadcast from smem.
-template <int R>
+// kPartial (deterministic variant): G is the split-major partial buffer [splits][Dp][R], stored with plain stores.
+template <int R, bool kPartial = false>
 __global__ void __launch_bounds__(128) lora_wgrad_kernel(const bf16* __restrict__ P, int64_t ldp, const bf16* __restrict__ Q,
                                                          int64_t ldq, float* __restrict__ G, int64_t gs_i, int64_t gs_j, int M,
                                                          int Dp, int rows_per_block) {
@@ -626,7 +639,10 @@ __global__ void __launch_bounds__(128) lora_wgrad_kernel(const bf16* __restrict_
   }
   if (i < Dp) {
 #pragma unroll
-    for (int j = 0; j < R; ++j) atomicAdd(G + (int64_t)i * gs_i + (int64_t)j * gs_j, acc[j]);
+    for (int j = 0; j < R; ++j) {
+      if constexpr (kPartial) G[((int64_t)blockIdx.y * Dp + i) * R + j] = acc[j];
+      else atomicAdd(G + (int64_t)i * gs_i + (int64_t)j * gs_j, acc[j]);
+    }
   }
 }
 
@@ -656,6 +672,8 @@ __global__ void __launch_bounds__(256) attn_delta_kernel(const bf16* __restrict_
 }
 
 // grads(fp32 accumulators) -> scale (1/world, clip) -> bf16 ; sumsq of the scaled-by-inv_world grads accumulated first
+// kPartial (deterministic variant): out[blockIdx.x] receives the CTA's share instead of an atomic add.
+template <bool kPartial = false>
 __global__ void __launch_bounds__(256) sumsq_kernel(const float* __restrict__ g, int64_t n, float pre_scale, float* __restrict__ out) {
   float acc = 0.f;
   for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x) {
@@ -669,7 +687,8 @@ __global__ void __launch_bounds__(256) sumsq_kernel(const float* __restrict__ g,
   if (threadIdx.x == 0) {
     float s = 0.f;
     for (int i = 0; i < 8; ++i) s += red[i];
-    atomicAdd(out, s);
+    if constexpr (kPartial) out[blockIdx.x] = s;
+    else atomicAdd(out, s);
   }
 }
 // out_bf16 = g * pre_scale * min(1, max_norm / (sqrt(sumsq) + 1e-6))     (torch.nn.utils.clip_grad_norm_ semantics)
@@ -682,6 +701,28 @@ __global__ void __launch_bounds__(256) clip_cast_kernel(const float* __restrict_
   }
   for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x)
     out[i] = __float2bfloat16_rn(g[i] * pre_scale * coef);
+}
+
+__global__ void __launch_bounds__(256) split_sum_kernel(const SplitSum S) {
+  const int64_t n = (int64_t)S.rows * S.cols;
+  for (int64_t e = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; e < n; e += (int64_t)gridDim.x * blockDim.x) {
+    const int row = (int)(e / S.cols), col = (int)(e - (int64_t)row * S.cols);
+    const int di = row / S.rows_per_dst + col / S.cols_per_dst;
+    float* d = di == 0 ? S.dst[0] : (di == 1 ? S.dst[1] : S.dst[2]);  // no dynamic index into the parameter: no local copy
+    if (d == nullptr) continue;
+    float acc = 0.f;
+    for (int sp = 0; sp < S.splits; ++sp) acc += S.part[sp * S.split_stride + e];
+    d += (int64_t)(row % S.rows_per_dst) * S.ld_row + (int64_t)(col % S.cols_per_dst) * S.ld_col;
+    *d = S.accumulate ? *d + acc : acc;
+  }
+}
+
+int launch_split_sum(const SplitSum& S, cudaStream_t stream) {
+  const int64_t n = (int64_t)S.rows * S.cols;
+  const int blocks = (int)(n < 256 * 1024 ? (n + 255) / 256 : 1024);
+  split_sum_kernel<<<blocks, 256, 0, stream>>>(S);
+  QFX_CUDA(cudaGetLastError());
+  return 0;
 }
 
 }  // namespace qfx
@@ -966,5 +1007,89 @@ __global__ void zero_rows_kernel(bf16* __restrict__ out, int64_t ld, int ncols, 
 extern "C" int qfx_zero_rows(void* out, int64_t ld, int ncols, const int* ranges, int n_ranges, void* stream) {
   QFX_CHECK_ARG(out && ranges && n_ranges > 0 && ncols % 8 == 0 && ld % 8 == 0, "qfx_zero_rows: bad arguments (ncols=%d)", ncols);
   zero_rows_kernel<<<2 * qfx::num_sms(), 256, 0, (cudaStream_t)stream>>>((bf16*)out, ld, ncols, ranges, n_ranges);
+  LAUNCH_OK();
+}
+
+// ---------------------------------------------------------------------------------------------------------------------
+// Deterministic variants (qfx.h): per-CTA partials into caller-owned scratch, then one fixed-order pass (launch_split_sum).
+extern "C" int qfx_mod_grad_det(const void* g, int64_t ldg, const void* m, int64_t ldm, const float* mean, const float* rstd,
+                                int rows_per_batch, float* sum_out, float* prod_out, int64_t ldo, int M, int D, float* scratch,
+                                int64_t scratch_floats, void* stream) {
+  QFX_CHECK_ARG(D % 8 == 0 && ldg % 8 == 0 && (m == nullptr || ldm % 8 == 0) && rows_per_batch > 0 && M % rows_per_batch == 0,
+                "qfx_mod_grad_det: bad dims (D=%d, M=%d, rows_per_batch=%d)", D, M, rows_per_batch);
+  QFX_CHECK_ARG((mean == nullptr) == (rstd == nullptr) && (mean == nullptr || m != nullptr), "qfx_mod_grad_det: mean/rstd need m");
+  const int B = M / rows_per_batch, cb = (D + 255) / 256;
+  int splits = (QFX_DET_MODGRAD_CTAS + cb * B - 1) / (cb * B);
+  splits = splits < 1 ? 1 : (splits > (rows_per_batch + 31) / 32 ? (rows_per_batch + 31) / 32 : splits);
+  const int64_t need = (int64_t)splits * 2 * B * D;
+  QFX_CHECK_ARG(scratch && scratch_floats >= need, "qfx_mod_grad_det: scratch holds %lld floats, needs %lld", (long long)scratch_floats,
+                (long long)need);
+  mod_grad_kernel<true><<<dim3(cb, B, splits), 256, 0, (cudaStream_t)stream>>>((const bf16*)g, ldg, (const bf16*)m, ldm, mean, rstd,
+                                                                              rows_per_batch, scratch, scratch, D, D);
+  QFX_CUDA(cudaGetLastError());
+  SplitSum S;
+  memset(&S, 0, sizeof(S));
+  S.part = scratch; S.split_stride = 2LL * B * D; S.splits = splits; S.rows = 2 * B; S.cols = D;
+  S.dst[0] = sum_out; S.dst[1] = m != nullptr ? prod_out : nullptr;
+  S.rows_per_dst = B; S.cols_per_dst = D; S.ld_row = ldo; S.ld_col = 1; S.accumulate = 1;
+  return launch_split_sum(S, (cudaStream_t)stream);
+}
+
+extern "C" int qfx_flow_loss_det(const void* pred, const void* x0, const void* noise, const float* w, float norm, float grad_scale,
+                                 float* loss, void* dpred, int B, int L, int Ltot, int C, float* scratch, int64_t scratch_floats,
+                                 void* stream) {
+  QFX_CHECK_ARG(loss && B > 0 && L > 0 && Ltot >= L && C > 0, "qfx_flow_loss_det: bad arguments");
+  QFX_CHECK_ARG(scratch && scratch_floats >= QFX_DET_LOSS_PARTIALS, "qfx_flow_loss_det: scratch holds %lld floats, needs %d",
+                (long long)scratch_floats, QFX_DET_LOSS_PARTIALS);
+  flow_loss_kernel<true><<<QFX_DET_LOSS_PARTIALS, 256, 0, (cudaStream_t)stream>>>(
+      (const bf16*)pred, (const bf16*)x0, (const bf16*)noise, w, norm, grad_scale, scratch, (bf16*)dpred, B, L, Ltot, C);
+  QFX_CUDA(cudaGetLastError());
+  SplitSum S;
+  memset(&S, 0, sizeof(S));
+  S.part = scratch; S.split_stride = 1; S.splits = QFX_DET_LOSS_PARTIALS; S.rows = S.cols = 1;
+  S.dst[0] = loss; S.rows_per_dst = S.cols_per_dst = 1; S.accumulate = 0;
+  return launch_split_sum(S, (cudaStream_t)stream);
+}
+
+extern "C" int qfx_lora_wgrad_det(const void* P, int64_t ldp, const void* Q, int64_t ldq, float* G, int64_t gs_i, int64_t gs_j, int M,
+                                  int Dp, int r, float* scratch, int64_t scratch_floats, void* stream) {
+  QFX_CHECK_ARG(r == 4 || r == 8 || r == 16 || r == 32 || r == 64, "qfx_lora_wgrad_det: rank %d unsupported (4/8/16/32/64)", r);
+  QFX_CHECK_ARG(G && M > 0 && Dp > 0, "qfx_lora_wgrad_det: bad arguments");
+  const int splits0 = (M + 511) / 512;
+  const int rows = ((M + splits0 - 1) / splits0 + 63) / 64 * 64;
+  const int splits = (M + rows - 1) / rows;
+  const int64_t need = (int64_t)splits * Dp * r;
+  QFX_CHECK_ARG(scratch && scratch_floats >= need, "qfx_lora_wgrad_det: scratch holds %lld floats, needs %lld", (long long)scratch_floats,
+                (long long)need);
+  dim3 grid((Dp + 127) / 128, splits);
+#define WGD(R)                                                                                                                    \
+  case R:                                                                                                                         \
+    lora_wgrad_kernel<R, true><<<grid, 128, 0, (cudaStream_t)stream>>>((const bf16*)P, ldp, (const bf16*)Q, ldq, scratch, 0, 0, M, \
+                                                                       Dp, rows);                                                 \
+    break;
+  switch (r) { WGD(4) WGD(8) WGD(16) WGD(32) WGD(64) }
+#undef WGD
+  QFX_CUDA(cudaGetLastError());
+  SplitSum S;
+  memset(&S, 0, sizeof(S));
+  S.part = scratch; S.split_stride = (int64_t)Dp * r; S.splits = splits; S.rows = Dp; S.cols = r;
+  S.dst[0] = G; S.rows_per_dst = Dp; S.cols_per_dst = r; S.ld_row = gs_i; S.ld_col = gs_j; S.accumulate = 1;
+  return launch_split_sum(S, (cudaStream_t)stream);
+}
+
+extern "C" int qfx_grad_finalize_det(const float* g, int64_t n, float pre_scale, float max_norm, float* sumsq, void* out_bf16,
+                                     float* scratch, int64_t scratch_floats, void* stream) {
+  QFX_CHECK_ARG(g && n > 0 && sumsq && out_bf16, "qfx_grad_finalize_det: bad arguments");
+  QFX_CHECK_ARG(scratch && scratch_floats >= QFX_DET_NORM_PARTIALS, "qfx_grad_finalize_det: scratch holds %lld floats, needs %d",
+                (long long)scratch_floats, QFX_DET_NORM_PARTIALS);
+  sumsq_kernel<true><<<QFX_DET_NORM_PARTIALS, 256, 0, (cudaStream_t)stream>>>(g, n, pre_scale, scratch);
+  QFX_CUDA(cudaGetLastError());
+  SplitSum S;
+  memset(&S, 0, sizeof(S));
+  S.part = scratch; S.split_stride = 1; S.splits = QFX_DET_NORM_PARTIALS; S.rows = S.cols = 1;
+  S.dst[0] = sumsq; S.rows_per_dst = S.cols_per_dst = 1; S.accumulate = 0;
+  int rc = launch_split_sum(S, (cudaStream_t)stream);
+  if (rc) return rc;
+  clip_cast_kernel<<<592, 256, 0, (cudaStream_t)stream>>>(g, n, pre_scale, sumsq, max_norm, (bf16*)out_bf16);
   LAUNCH_OK();
 }

@@ -36,4 +36,19 @@ int make_tmap_f32(CUtensorMap* out, const void* base, int rank, const uint64_t* 
 
 int num_sms();
 
+// Fixed-order reduction of per-CTA partials (the deterministic entry points): element e = (row, col) of a rows x cols grid is
+//   acc = part[0*split_stride + e] + part[1*split_stride + e] + ... (split order)
+// and goes to dst[row / rows_per_dst + col / cols_per_dst][(row % rows_per_dst) * ld_row + (col % cols_per_dst) * ld_col]
+// (+= when accumulate, else =); a NULL dst skips its elements.  One thread per element: no atomics.
+struct SplitSum {
+  const float* part;
+  int64_t split_stride;
+  int splits, rows, cols;
+  float* dst[3];
+  int rows_per_dst, cols_per_dst;
+  int64_t ld_row, ld_col;
+  int accumulate;
+};
+int launch_split_sum(const SplitSum& S, cudaStream_t stream);  // elementwise.cu
+
 }  // namespace qfx

@@ -13,6 +13,8 @@
 
 namespace qfx {
 
+// kPartial (deterministic variant): out[blockIdx.x] receives the CTA's share instead of an atomic add.
+template <bool kPartial = false>
 __global__ void __launch_bounds__(256) adamw_sumsq_kernel(const float* __restrict__ g, int64_t n, float pre_scale, float* __restrict__ out) {
   float acc = 0.f;
   for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x) {
@@ -27,7 +29,8 @@ __global__ void __launch_bounds__(256) adamw_sumsq_kernel(const float* __restric
   if (threadIdx.x == 0) {
     float s = 0.f;
     for (int i = 0; i < 8; ++i) s += red[i];
-    atomicAdd(out, s);
+    if constexpr (kPartial) out[blockIdx.x] = s;
+    else atomicAdd(out, s);
   }
 }
 
@@ -76,6 +79,32 @@ extern "C" int qfx_fused_adamw(const qfx_adamw_tensor* tensors_dev, const int* c
   QFX_CUDA(cudaMemsetAsync(sumsq, 0, sizeof(float), st));
   adamw_sumsq_kernel<<<4 * num_sms(), 256, 0, st>>>(grad, n_grad, pre_scale, sumsq);
   QFX_CUDA(cudaGetLastError());
+  const float bc1 = 1.f - powf(beta1, (float)step), bc2 = 1.f - powf(beta2, (float)step);
+  fused_adamw_kernel<<<n_chunks, 256, 0, st>>>(tensors_dev, reinterpret_cast<const int2*>(chunks_dev), grad, exp_avg, exp_avg_sq, sumsq,
+                                              pre_scale, max_norm, lr, beta1, beta2, eps, weight_decay, bc1, sqrtf(bc2));
+  QFX_CUDA(cudaGetLastError());
+  return 0;
+}
+
+/* Deterministic variant: QFX_DET_NORM_PARTIALS per-CTA shares of ||grad * pre_scale||^2 go to `scratch` and are summed in a fixed
+ * order into sumsq before the update kernel reads it. */
+extern "C" int qfx_fused_adamw_det(const qfx_adamw_tensor* tensors_dev, const int* chunks_dev, int n_chunks, const float* grad,
+                                   int64_t n_grad, float* exp_avg, float* exp_avg_sq, float* sumsq, float pre_scale, float max_norm,
+                                   float lr, float beta1, float beta2, float eps, float weight_decay, int step, float* scratch,
+                                   int64_t scratch_floats, void* stream) {
+  QFX_CHECK_ARG(tensors_dev && chunks_dev && n_chunks > 0 && grad && exp_avg && exp_avg_sq && sumsq && step >= 1,
+                "qfx_fused_adamw_det: bad arguments");
+  QFX_CHECK_ARG(scratch && scratch_floats >= QFX_DET_NORM_PARTIALS, "qfx_fused_adamw_det: scratch holds %lld floats, needs %d",
+                (long long)scratch_floats, QFX_DET_NORM_PARTIALS);
+  cudaStream_t st = (cudaStream_t)stream;
+  adamw_sumsq_kernel<true><<<QFX_DET_NORM_PARTIALS, 256, 0, st>>>(grad, n_grad, pre_scale, scratch);
+  QFX_CUDA(cudaGetLastError());
+  SplitSum S;
+  memset(&S, 0, sizeof(S));
+  S.part = scratch; S.split_stride = 1; S.splits = QFX_DET_NORM_PARTIALS; S.rows = S.cols = 1;
+  S.dst[0] = sumsq; S.rows_per_dst = S.cols_per_dst = 1; S.accumulate = 0;
+  int rc = launch_split_sum(S, st);
+  if (rc) return rc;
   const float bc1 = 1.f - powf(beta1, (float)step), bc2 = 1.f - powf(beta2, (float)step);
   fused_adamw_kernel<<<n_chunks, 256, 0, st>>>(tensors_dev, reinterpret_cast<const int2*>(chunks_dev), grad, exp_avg, exp_avg_sq, sumsq,
                                               pre_scale, max_norm, lr, beta1, beta2, eps, weight_decay, bc1, sqrtf(bc2));

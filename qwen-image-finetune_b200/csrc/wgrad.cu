@@ -24,6 +24,7 @@ struct WgradParams {
   float* G[WG_MAXG];
   int64_t gs_i, gs_j;
   int M, Na, ng, mode, Dg, r, rows_per_split;
+  float* part;  // deterministic variant: split-major partial tiles [splits][Na][NG * r]
 };
 
 template <int NG>
@@ -33,7 +34,8 @@ __device__ __forceinline__ void wgmma_wgrad(float* d, uint64_t a, uint64_t b, in
   else wgmma_ss_n192<1, 1>(d, a, b, scale_d);
 }
 
-template <int NG>
+// kPartial: each CTA stores its partial tile with plain stores into P.part (reduced in split order by launch_split_sum)
+template <int NG, bool kPartial = false>
 __global__ void __launch_bounds__(384, 1) wgrad_kernel(const __grid_constant__ WgradParams P) {
   constexpr int A_BYTES = 2 * 8192, B_BYTES = NG * 8192, STAGE = A_BYTES + B_BYTES, STAGES = 4;
   extern __shared__ uint8_t smem_raw[];
@@ -107,7 +109,9 @@ __global__ void __launch_bounds__(384, 1) wgrad_kernel(const __grid_constant__ W
           for (int e = 0; e < 2; ++e) {
             const int col = 8 * jj + 2 * (l & 3) + e;
             const int g = col >> 6, j = col & 63;
-            if (j < P.r) {
+            if (kPartial && j < P.r) {
+              P.part[((int64_t)blockIdx.y * P.Na + i) * (NG * P.r) + g * P.r + j] = acc[4 * jj + 2 * h + e];
+            } else if (j < P.r) {
               const int gg = P.mode == 1 ? grp : g;
               const int64_t ii = P.mode == 1 ? (int64_t)(i - grp * P.Dg) : (int64_t)i;
               atomicAdd(P.G[gg] + ii * P.gs_i + (int64_t)j * P.gs_j, acc[4 * jj + 2 * h + e]);
@@ -119,15 +123,15 @@ __global__ void __launch_bounds__(384, 1) wgrad_kernel(const __grid_constant__ W
   }
 }
 
-template <int NG>
+template <int NG, bool kPartial = false>
 static int launch_wgrad(const WgradParams& P, dim3 grid, cudaStream_t st) {
   constexpr int SMEM = 4 * (2 * 8192 + NG * 8192) + 1024 + 256;
   static bool done = false;
   if (!done) {
-    QFX_CUDA(cudaFuncSetAttribute(wgrad_kernel<NG>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM));
+    QFX_CUDA(cudaFuncSetAttribute(wgrad_kernel<NG, kPartial>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM));
     done = true;
   }
-  wgrad_kernel<NG><<<grid, 384, SMEM, st>>>(P);
+  wgrad_kernel<NG, kPartial><<<grid, 384, SMEM, st>>>(P);
   QFX_CUDA(cudaGetLastError());
   return 0;
 }
@@ -174,4 +178,60 @@ extern "C" int qfx_lora_wgrad_tc(const void* A, int64_t lda, int Na, const void*
     case 2: return launch_wgrad<2>(P, grid, st);
     default: return launch_wgrad<3>(P, grid, st);
   }
+}
+
+/* Deterministic variant: the same operation and row split, but every CTA stores its [128 x NG*r] partial into `scratch` and one
+ * fixed-order pass adds the partials into Gp.  The split count depends on the shapes only (not on the GPU):
+ *   splits = max(1, min(ceil(M / 256), ceil(QFX_DET_WGRAD_CTAS / (Na / 128)))),  rows = ceil(ceil(M / splits) / 64) * 64,
+ *   scratch_floats >= ceil(M / rows) * Na * NG * r,  NG = (mode == 1 ? 1 : G). */
+extern "C" int qfx_lora_wgrad_tc_det(const void* A, int64_t lda, int Na, const void* B, int64_t ldb, int G, int M, int mode, int Dg,
+                                     float* const* Gp, int64_t gs_i, int64_t gs_j, int r, float* scratch, int64_t scratch_floats,
+                                     void* stream) {
+  QFX_CHECK_ARG(G >= 1 && G <= WG_MAXG && r >= 1 && r <= 64 && M > 0 && Na % 128 == 0 && Na > 0, "qfx_lora_wgrad_tc_det: bad shape");
+  QFX_CHECK_ARG(mode == 0 || (mode == 1 && Dg % 128 == 0 && Na == G * Dg), "qfx_lora_wgrad_tc_det: bad mode/Dg");
+  QFX_CHECK_ARG(lda % 8 == 0 && ldb % 8 == 0, "qfx_lora_wgrad_tc_det: leading dims must be multiples of 8");
+  const int tiles = Na / 128, ng = mode == 1 ? 1 : G;
+  int splits = (QFX_DET_WGRAD_CTAS + tiles - 1) / tiles;
+  const int max_splits = (M + 255) / 256;
+  if (splits > max_splits) splits = max_splits;
+  if (splits < 1) splits = 1;
+  const int rows = ((M + splits - 1) / splits + 63) / 64 * 64;
+  splits = (M + rows - 1) / rows;
+  const int64_t need = (int64_t)splits * Na * ng * r;
+  QFX_CHECK_ARG(scratch && scratch_floats >= need, "qfx_lora_wgrad_tc_det: scratch holds %lld floats, needs %lld",
+                (long long)scratch_floats, (long long)need);
+  WgradParams P;
+  memset(&P, 0, sizeof(P));
+  {
+    uint64_t dims[2] = {(uint64_t)Na, (uint64_t)M};
+    uint64_t str[1] = {(uint64_t)lda * 2};
+    uint32_t box[2] = {64, 64};
+    int rc = make_tmap_bf16(&P.tmA, A, 2, dims, str, box);
+    if (rc) return rc;
+    uint64_t dimsb[2] = {(uint64_t)(64 * G), (uint64_t)M};
+    uint64_t strb[1] = {(uint64_t)ldb * 2};
+    rc = make_tmap_bf16(&P.tmB, B, 2, dimsb, strb, box);
+    if (rc) return rc;
+  }
+  for (int g = 0; g < G; ++g) P.G[g] = Gp[g];
+  P.part = scratch;
+  P.gs_i = gs_i; P.gs_j = gs_j; P.M = M; P.Na = Na; P.ng = G; P.mode = mode; P.Dg = Dg; P.r = r;
+  P.rows_per_split = rows;
+  const dim3 grid(tiles, splits);
+  cudaStream_t st = (cudaStream_t)stream;
+  int rc;
+  switch (ng) {
+    case 1: rc = launch_wgrad<1, true>(P, grid, st); break;
+    case 2: rc = launch_wgrad<2, true>(P, grid, st); break;
+    default: rc = launch_wgrad<3, true>(P, grid, st); break;
+  }
+  if (rc) return rc;
+  SplitSum S;
+  memset(&S, 0, sizeof(S));
+  S.part = scratch; S.split_stride = (int64_t)Na * ng * r; S.splits = splits; S.rows = Na; S.cols = ng * r;
+  for (int g = 0; g < G; ++g) S.dst[g] = Gp[g];
+  S.rows_per_dst = mode == 1 ? Dg : Na;  // mode 1: A-column group g -> Gp[g];  mode 0: column group g -> Gp[g]
+  S.cols_per_dst = r;
+  S.ld_row = gs_i; S.ld_col = gs_j; S.accumulate = 1;
+  return launch_split_sum(S, st);
 }

@@ -158,7 +158,9 @@ class FluxB200(FusedMMDiTBase):
         D = self.D
         extra = [(k, (B, 256)) for k in ("sin", "gsin")] + [(k, (B, D)) for k in ("e1", "temb", "gemb", "pemb")]
         extra += [("mods", (B, self.L * 2 * 6 * D)), ("smods", (B, max(self.Ls, 1) * 3 * D)), ("fmod", (B, 2 * D))]
-        return self._get_workspace((B, T, Limg, train), lambda: self._alloc_common({}, B, T, Limg, train, self.L, self.Ls, extra=extra))
+        det = train and torch.are_deterministic_algorithms_enabled()  # read on every forward: selects the fixed-order backward
+        return self._get_workspace((B, T, Limg, train, det),
+                                   lambda: self._alloc_common({}, B, T, Limg, train, self.L, self.Ls, extra=extra, det=det))
 
     # ------------------------------------------------------------------------------------------------ single block
     def _single_fwd(self, ws, l, Xin, Xout, save, recompute=False):
@@ -185,7 +187,7 @@ class FluxB200(FusedMMDiTBase):
         dsm = lambda j: self._dmod(ws, "sgl", l, j)  # d(shift, scale, gate): ONE vector per sample for text and image rows alike
         if dsm(2) is not None:
             for s in (0, 1):
-                lib.mod_grad(self._rows(ws, dX, s), self._rpb(ws, s), m=self._rows(ws, save["y_out"], s), prod_out=dsm(2))
+                self._mod_grad(ws, self._rows(ws, dX, s), self._rpb(ws, s), m=self._rows(ws, save["y_out"], s), prod_out=dsm(2))
         # d[attn | mlp] = dY . W_out (+ U . A_lora)   (dY = dX * gate is already in ws['dY']); the two column ranges of the
         # concatenated input go to different consumers (attention backward / GELU backward), so they are two contractions
         pa, pm = [], []
@@ -207,8 +209,8 @@ class FluxB200(FusedMMDiTBase):
         self._dgrad_grouped(ws, l, "s_mlp", ws["dbig"], ws["dxm"], D, 4 * D, 4 * D, ws["xm"], epilogue=lib.EPI_ADD, resid=ws["dxm"])
         for s in (0, 1):
             if dsm(0) is not None:
-                lib.mod_grad(self._rows(ws, ws["dxm"], s), self._rpb(ws, s), sum_out=dsm(0), m=self._rows(ws, Xin, s),
-                             prod_out=dsm(1), mean=self._rows(ws, st[0], s), rstd=self._rows(ws, st[1], s))
+                self._mod_grad(ws, self._rows(ws, ws["dxm"], s), self._rpb(ws, s), sum_out=dsm(0), m=self._rows(ws, Xin, s),
+                               prod_out=dsm(1), mean=self._rows(ws, st[0], s), rstd=self._rows(ws, st[1], s))
         self._ln_bwd2(ws, ws["dxm"], Xin, st[0], st[1], self._smod(ws, l, 1), dXn, dres=dX, gate=prev_gate, dx_gated=ws["dY"])
 
     # ------------------------------------------------------------------------------------------------ forward

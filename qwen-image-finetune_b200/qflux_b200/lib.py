@@ -24,7 +24,8 @@ class QfxError(RuntimeError):
 
 
 LAUNCHES = 0  # kernels of THIS library launched so far (bench.py reports the per-step delta as gpu_launches)
-_KERNELS_PER_CALL = {"qfx_grad_finalize": 2}
+_KERNELS_PER_CALL = {"qfx_grad_finalize": 2, "qfx_attn_bwd_det": 2, "qfx_lora_wgrad_tc_det": 2, "qfx_lora_wgrad_det": 2,
+                     "qfx_mod_grad_det": 2, "qfx_flow_loss_det": 2, "qfx_grad_finalize_det": 3, "qfx_fused_adamw_det": 3}
 
 
 def check(rc: int, what: str):
@@ -437,6 +438,104 @@ def attn_fwd(Q, K, V, out_txt, out_img, split, lse=None, kv_len=None, scale=None
     scale = scale if scale is not None else d ** -0.5
     check(_attn_fwd(ptr(Q), ptr(K), ptr(V), ptr(out_txt), _ld(out_txt), split, ptr(out_img), _ld(out_img), S - split, split,
                     ptr(lse), ptr(kv_len), ptr(txt_len), B, H, S, scale, cur_stream()), "qfx_attn_fwd")
+
+
+# ---------------------------------------------------------------------------------------------------- deterministic variants
+# Picked by the model under torch.use_deterministic_algorithms(True): the same operations without floating-point atomics (qfx.h).
+# The reductions take caller-owned fp32 scratch; the det_scratch_* rules below restate qfx.h's size rules (the C side refuses less).
+DET_WGRAD_CTAS, DET_MODGRAD_CTAS, DET_LOSS_PARTIALS, DET_NORM_PARTIALS = 264, 528, 296, 592
+
+
+def _cdiv(a, b):
+    return -(-a // b)
+
+
+def det_scratch_wgrad_tc(M, Na, ng, r):
+    """fp32 scratch of qfx_lora_wgrad_tc_det; ng = 1 for mode 1, else the number of groups."""
+    splits = max(1, min(_cdiv(M, 256), _cdiv(DET_WGRAD_CTAS, Na // 128)))
+    rows = _cdiv(_cdiv(M, splits), 64) * 64
+    return _cdiv(M, rows) * Na * ng * r
+
+
+def det_scratch_wgrad(M, Dp, r):
+    rows = _cdiv(_cdiv(M, _cdiv(M, 512)), 64) * 64
+    return _cdiv(M, rows) * Dp * r
+
+
+def det_scratch_mod_grad(M, rows_per_batch, D):
+    B = M // rows_per_batch
+    cb = _cdiv(D, 256)
+    splits = max(1, min(_cdiv(rows_per_batch, 32), _cdiv(DET_MODGRAD_CTAS, cb * B)))
+    return splits * 2 * B * D
+
+
+def _scratch(t):
+    assert t.dtype == torch.float32 and t.is_contiguous()
+    return ptr(t), t.numel()
+
+
+_attn_bwd_det = _sig("qfx_attn_bwd_det", _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _f, _vp)
+_wgrad_tc_det = _sig("qfx_lora_wgrad_tc_det", _vp, _i64, _i, _vp, _i64, _i, _i, _i, _i, C.POINTER(C.c_void_p), _i64, _i64, _i, _vp,
+                     _i64, _vp)
+_wgrad_det = _sig("qfx_lora_wgrad_det", _vp, _i64, _vp, _i64, _vp, _i64, _i64, _i, _i, _i, _vp, _i64, _vp)
+_mod_grad_det = _sig("qfx_mod_grad_det", _vp, _i64, _vp, _i64, _vp, _vp, _i, _vp, _vp, _i64, _i, _i, _vp, _i64, _vp)
+_floss_det = _sig("qfx_flow_loss_det", _vp, _vp, _vp, _vp, _f, _f, _vp, _vp, _i, _i, _i, _i, _vp, _i64, _vp)
+_gfin_det = _sig("qfx_grad_finalize_det", _vp, _i64, _f, _f, _vp, _vp, _vp, _i64, _vp)
+_adamw_det = _sig("qfx_fused_adamw_det", _vp, _vp, _i, _vp, _i64, _vp, _vp, _vp, _f, _f, _f, _f, _f, _f, _f, _i, _vp, _i64, _vp)
+
+
+def attn_bwd_det(Q, K, V, dO, lse, delta, dQ_accum, dK, dV, kv_len=None, scale=None, txt_len=None, split=0):
+    """attn_bwd without atomics: dQ_accum (prefilled by the caller) receives every element once."""
+    require_cuda(Q, K, V, dO, lse, delta, dQ_accum, dK, dV, kv_len, txt_len)
+    B, H, S, d = Q.shape
+    assert d == 128 and dQ_accum.dtype == torch.float32
+    scale = scale if scale is not None else d ** -0.5
+    check(_attn_bwd_det(ptr(Q), ptr(K), ptr(V), ptr(dO), ptr(lse), ptr(delta), ptr(dQ_accum), ptr(dK), ptr(dV), ptr(kv_len),
+                        ptr(txt_len), split, B, H, S, scale, cur_stream()), "qfx_attn_bwd_det")
+
+
+def lora_wgrad_tc_det(A, B, G_list, gs_i, gs_j, r, mode=0, Dg=0, *, scratch):
+    require_cuda(A, B, scratch, *G_list)
+    n = len(G_list)
+    arr = (C.c_void_p * n)(*[g.data_ptr() for g in G_list])
+    check(_wgrad_tc_det(ptr(A), A.stride(0), A.shape[1], ptr(B), B.stride(0), n, A.shape[0], mode, Dg, arr, gs_i, gs_j, r,
+                        *_scratch(scratch), cur_stream()), "qfx_lora_wgrad_tc_det")
+
+
+def lora_wgrad_det(P, Q, G, gs_i, gs_j, r, *, scratch):
+    require_cuda(P, Q, G, scratch)
+    check(_wgrad_det(ptr(P), P.stride(0), ptr(Q), Q.stride(0), ptr(G), gs_i, gs_j, P.shape[0], P.shape[1], r, *_scratch(scratch),
+                     cur_stream()), "qfx_lora_wgrad_det")
+
+
+def mod_grad_det(g, rows_per_batch, sum_out=None, m=None, prod_out=None, mean=None, rstd=None, *, scratch):
+    require_cuda(g, m, sum_out, prod_out, mean, rstd, scratch)
+    o = sum_out if sum_out is not None else prod_out
+    assert o.dtype == torch.float32 and (sum_out is None or prod_out is None or sum_out.stride(0) == prod_out.stride(0))
+    check(_mod_grad_det(ptr(g), g.stride(0), ptr(m), _ld(m), ptr(mean), ptr(rstd), rows_per_batch, ptr(sum_out), ptr(prod_out),
+                        o.stride(0), g.shape[0], g.shape[1], *_scratch(scratch), cur_stream()), "qfx_mod_grad_det")
+
+
+def flow_loss_det(pred, x0, noise, w, norm, loss, dpred=None, grad_scale=1.0, *, scratch):
+    require_cuda(pred, x0, noise, w, loss, dpred, scratch)
+    B, L, Cc = x0.shape
+    check(_floss_det(ptr(pred), ptr(x0), ptr(noise), ptr(w), norm, grad_scale, ptr(loss), ptr(dpred), B, L, pred.shape[1], Cc,
+                     *_scratch(scratch), cur_stream()), "qfx_flow_loss_det")
+
+
+def grad_finalize_det(g_f32, pre_scale, max_norm, sumsq, out_bf16, *, scratch):
+    require_cuda(g_f32, sumsq, out_bf16, scratch)
+    check(_gfin_det(ptr(g_f32), g_f32.numel(), pre_scale, max_norm, ptr(sumsq), ptr(out_bf16), *_scratch(scratch), cur_stream()),
+          "qfx_grad_finalize_det")
+
+
+def fused_adamw_det(tables, grad, exp_avg, exp_avg_sq, sumsq, pre_scale, max_norm, lr, beta1, beta2, eps, weight_decay, step, *,
+                    scratch):
+    raw, chunks = tables
+    require_cuda(raw, chunks, grad, exp_avg, exp_avg_sq, sumsq, scratch)
+    check(_adamw_det(ptr(raw), ptr(chunks), chunks.shape[0], ptr(grad), grad.numel(), ptr(exp_avg), ptr(exp_avg_sq), ptr(sumsq),
+                     float(pre_scale), float(max_norm), float(lr), float(beta1), float(beta2), float(eps), float(weight_decay),
+                     int(step), *_scratch(scratch), cur_stream()), "qfx_fused_adamw_det")
 
 
 # ---------------------------------------------------------------------------------------------------- NF4 frozen weights (nf4.py)

@@ -640,6 +640,7 @@ class FusedMMDiTBase(nn.Module):
         self.G32 = torch.zeros(off, device=self.dev, dtype=torch.float32)
         self.G16 = torch.zeros(off, device=self.dev, dtype=BF)
         self._gnorm_sq = torch.zeros(1, device=self.dev, dtype=torch.float32)
+        self._gnorm_parts = torch.zeros(lib.DET_NORM_PARTIALS, device=self.dev, dtype=torch.float32)  # deterministic finalize
         self._gscratch = torch.zeros(5 * self.D * PAD, device=self.dev, dtype=torch.float32)
         self._ws = self._ws_key = None  # per-block saved tensors depend on which sites exist
         self._train_ws, self._infer_ws = None, {}
@@ -863,7 +864,10 @@ class FusedMMDiTBase(nn.Module):
 
     def finalize_grads(self, world_size: int = 1, max_norm: float = 0.0):
         """fp32 accumulator (already all-reduced by the caller) -> mean over ranks -> clip -> bf16 `param.grad`."""
-        lib.grad_finalize(self.G32, 1.0 / world_size, max_norm, self._gnorm_sq, self.G16)
+        if torch.are_deterministic_algorithms_enabled():
+            lib.grad_finalize_det(self.G32, 1.0 / world_size, max_norm, self._gnorm_sq, self.G16, scratch=self._gnorm_parts)
+        else:
+            lib.grad_finalize(self.G32, 1.0 / world_size, max_norm, self._gnorm_sq, self.G16)
         self.bind_param_grads()
         return self._gnorm_sq
 
@@ -874,6 +878,13 @@ class FusedMMDiTBase(nn.Module):
 
     def _rpb(self, ws, s):
         return ws["Limg"] if s == 0 else ws["T"]
+
+    def _mod_grad(self, ws, g, rows_per_batch, **kw):
+        """lib.mod_grad, or its fixed-order variant in a deterministic workspace."""
+        if ws["det"]:
+            lib.mod_grad_det(g, rows_per_batch, scratch=ws["det_scratch"], **kw)
+        else:
+            lib.mod_grad(g, rows_per_batch, **kw)
 
     def _plan_bands(self, ws, valid_img_rows):
         """Pad-to-max multi-resolution batch: the block GEMMs compute only the 256-row bands that hold valid image rows of a
@@ -1022,12 +1033,14 @@ class FusedMMDiTBase(nn.Module):
             else:  # slot without an adapter (e.g. LoRA on to_q/to_v only): its zero factors produce zeros -> scratch
                 gB.append(self._gscratch)
                 gA.append(self._gscratch)
-        lib.lora_wgrad_tc(dY, Tb, gB, r, 1, r, mode=1 if site.n > 1 else 0, Dg=n_out_each if site.n > 1 else 0)
+        det = {"scratch": ws["det_scratch"]} if ws["det"] else {}
+        wgrad_tc = lib.lora_wgrad_tc_det if det else lib.lora_wgrad_tc
+        wgrad_tc(dY, Tb, gB, r, 1, r, mode=1 if site.n > 1 else 0, Dg=n_out_each if site.n > 1 else 0, **det)
         if Xsaved.shape[1] % 128 == 0:
-            lib.lora_wgrad_tc(Xsaved, U, gA, 1, Xsaved.shape[1], r, mode=0)
+            wgrad_tc(Xsaved, U, gA, 1, Xsaved.shape[1], r, mode=0, **det)
         else:  # 64-channel latent embedder: too narrow for the wgmma tile, a [r, 64] result on the CUDA cores
             for g in range(site.n):
-                lib.lora_wgrad(Xsaved, U[:, g * PAD:(g + 1) * PAD], gA[g], 1, Xsaved.shape[1], r)
+                (lib.lora_wgrad_det if det else lib.lora_wgrad)(Xsaved, U[:, g * PAD:(g + 1) * PAD], gA[g], 1, Xsaved.shape[1], r, **det)
         return U, site.A_pad, site.n
 
     def _lora_bwd(self, ws, l, grp, s, dY, Xsaved, n_out_each):
@@ -1128,8 +1141,8 @@ class FusedMMDiTBase(nn.Module):
         if not (consumer_clears and ws.get("dQ_clean")):
             ws["dQ"].zero_()
         ws["dQ_clean"] = False
-        lib.attn_bwd(Qs, Ks, Vs, ws["dOj"], lse, ws["delta"], ws["dQ"], ws["dK"], ws["dV"], kv_len=ws.get("kv_len"),
-                     txt_len=ws.get("txt_len"), split=T)
+        (lib.attn_bwd_det if ws["det"] else lib.attn_bwd)(Qs, Ks, Vs, ws["dOj"], lse, ws["delta"], ws["dQ"], ws["dK"], ws["dV"],
+                                                          kv_len=ws.get("kv_len"), txt_len=ws.get("txt_len"), split=T)
         lib.qk_norm_rope_bwd_pair(ws["dQ"], ws["dK"], ws["dV"], qkv, g_txt, g_img, Mt, ws["rope"], ws["dqkv"], round_mid=self.round_mid,
                                   clear_dq=consumer_clears)
         ws["dQ_clean"] = consumer_clears
@@ -1143,7 +1156,7 @@ class FusedMMDiTBase(nn.Module):
         dm = lambda s, j: self._dmod(ws, "dbl", 2 * l + s, j)  # fp32 [B, D] accumulators of d(shift1, scale1, gate1, shift2, scale2, gate2)
         for s in (0, 1):
             if dm(s, 5) is not None:  # d gate2 = sum_t dXout * mlp_out  (before dX is overwritten with dXmid below)
-                lib.mod_grad(self._rows(ws, dX, s), self._rpb(ws, s), m=self._rows(ws, save["y_mlp"], s), prod_out=dm(s, 5))
+                self._mod_grad(ws, self._rows(ws, dX, s), self._rpb(ws, s), m=self._rows(ws, save["y_mlp"], s), prod_out=dm(s, 5))
         # ---- MLP branch
         self._dgrad_grouped(ws, l, "down", ws["dY"], ws["dbig"], 4 * D, D, D, save.get("h"), epilogue=lib.EPI_DGELU, aux=u)
         if self._site(l, "up", 0) or self._site(l, "up", 1):  # LoRA input = xm2, recomputed from the statistics
@@ -1152,14 +1165,14 @@ class FusedMMDiTBase(nn.Module):
         # ---- norm2 backward: dXmid = dX + LN_bwd ; also emit dXmid * gate1 for the attention out-projection
         for s in (0, 1):
             if dm(s, 3) is not None:  # d shift2 = sum_t dy ; d scale2 = sum_t dy * LN(xmid)
-                lib.mod_grad(self._rows(ws, ws["dxm"], s), self._rpb(ws, s), sum_out=dm(s, 3), m=self._rows(ws, xmid, s),
-                             prod_out=dm(s, 4), mean=self._rows(ws, st[2], s), rstd=self._rows(ws, st[3], s))
+                self._mod_grad(ws, self._rows(ws, ws["dxm"], s), self._rpb(ws, s), sum_out=dm(s, 3), m=self._rows(ws, xmid, s),
+                               prod_out=dm(s, 4), mean=self._rows(ws, st[2], s), rstd=self._rows(ws, st[3], s))
         T, Limg, Mt = ws["T"], ws["Limg"], ws["Mt"]
         lib.ln_modulate_bwd_pair(ws["dxm"], xmid, st[2], st[3], (mods(4)[1], T, mods(2)[1]), (mods(4)[0], Limg, mods(2)[0]), Mt, dX,
                                  dres=dX, dx_gated=ws["dY"])
         for s in (0, 1):
             if dm(s, 2) is not None:  # d gate1 = sum_t dXmid * attn_out   (dX holds dXmid now)
-                lib.mod_grad(self._rows(ws, dX, s), self._rpb(ws, s), m=self._rows(ws, save["y_attn"], s), prod_out=dm(s, 2))
+                self._mod_grad(ws, self._rows(ws, dX, s), self._rpb(ws, s), m=self._rows(ws, save["y_attn"], s), prod_out=dm(s, 2))
         # ---- attention output projection (LoRA input = O), attention, q|k|v projection (LoRA input = xm1, recomputed)
         lbs = self._lora_bwd_pair(ws, l, "out", ws["dY"], O, D)
         self._dgrad_attn_out(ws, [(self._rows(ws, ws["dY"], s), self._wb(l, "out", s)[0],
@@ -1174,8 +1187,8 @@ class FusedMMDiTBase(nn.Module):
         # ---- norm1 backward: dXin = dXmid + LN_bwd ; emit dXin * (gate of the block before)
         for s in (0, 1):
             if dm(s, 0) is not None:
-                lib.mod_grad(self._rows(ws, ws["dxm"], s), self._rpb(ws, s), sum_out=dm(s, 0), m=self._rows(ws, Xin, s),
-                             prod_out=dm(s, 1), mean=self._rows(ws, st[0], s), rstd=self._rows(ws, st[1], s))
+                self._mod_grad(ws, self._rows(ws, ws["dxm"], s), self._rpb(ws, s), sum_out=dm(s, 0), m=self._rows(ws, Xin, s),
+                               prod_out=dm(s, 1), mean=self._rows(ws, st[0], s), rstd=self._rows(ws, st[1], s))
         pg = prev_gate if prev_gate else (None, None)
         lib.ln_modulate_bwd_pair(ws["dxm"], Xin, st[0], st[1], (mods(1)[1], T, pg[1]), (mods(1)[0], Limg, pg[0]), Mt, dXn, dres=dX,
                                  dx_gated=ws["dY"] if prev_gate else None)
@@ -1290,9 +1303,24 @@ class FusedMMDiTBase(nn.Module):
             ent.append((1, "y_out", (M, D), BF))
         return ent
 
-    def _fixed_entries(self, B, T, Limg, train, nblk, extra):
+    def _det_scratch_floats(self, B, T, Limg):
+        """fp32 scratch of the deterministic reductions of one training step: the largest need over the loss, every modulation-gradient
+        row group and every LoRA site's weight gradients (lib.det_scratch_* restate qfx.h's rules)."""
+        S = T + Limg
+        n = lib.DET_LOSS_PARTIALS
+        for M, rpb in ((B * Limg, Limg), (B * T, T), (B * S, S)):
+            n = max(n, lib.det_scratch_mod_grad(M, rpb, self.D))
+        for site in self.sites.values():
+            d_in, d_out = site.A_pad.shape[1], site.B_pad.shape[0] // site.n
+            for M in (B * Limg, B * T, B * S):
+                n = max(n, lib.det_scratch_wgrad_tc(M, site.n * d_out, 1, site.r))
+                n = max(n, lib.det_scratch_wgrad_tc(M, d_in, site.n, site.r) if d_in % 128 == 0 else lib.det_scratch_wgrad(M, d_in, site.r))
+        return n
+
+    def _fixed_entries(self, B, T, Limg, train, nblk, extra, det=False):
         """([(name, shape, dtype)] allocated before the saved dicts, [...] after them): every workspace buffer whose size does
-        not depend on the activation plan.  `extra`: the family's conditioning buffers [(name, shape)] (bf16), allocated last."""
+        not depend on the activation plan.  `extra`: the family's conditioning buffers [(name, shape)] (bf16), allocated last.
+        det: the step runs the deterministic kernels, whose reduction scratch is one more fixed buffer."""
         D, H, S, Mi, f32 = self.D, self.H, T + Limg, B * Limg, torch.float32
         M = B * S
         pre = [("X", (nblk + 1 if train else 2, M, D), BF), ("xm", (M, D), BF), ("h", (M, 4 * D), BF),
@@ -1304,6 +1332,8 @@ class FusedMMDiTBase(nn.Module):
                      ("dOj", (B, H, S, 128), BF), ("dK", (B, H, S, 128), BF), ("dV", (B, H, S, 128), BF), ("dQ", (B, H, S, 128), f32),
                      ("delta", (B, H, S), f32), ("U", (M, 3 * PAD), BF), ("dhn", (Mi, D), BF), ("dpred", (Mi, self.C_out), BF),
                      ("loss", (1,), f32)]
+            if det:
+                post.append(("det_scratch", (self._det_scratch_floats(B, T, Limg),), f32))
         return pre, post + [(k, s, BF) for k, s in extra]
 
     def _activation_limit_now(self):
@@ -1313,7 +1343,7 @@ class FusedMMDiTBase(nn.Module):
             return None
         return torch.cuda.mem_get_info(self.dev)[0] - ACTIVATION_HEADROOM
 
-    def _alloc_common(self, ws, B, T, Limg, train, n_double, n_single=0, extra=()):
+    def _alloc_common(self, ws, B, T, Limg, train, n_double, n_single=0, extra=(), det=False):
         """The workspace of one (B, T, Limg, train) shape.  Training: every block either keeps its own saved dict or, when the
         activation plan recomputes it, points at the one scratch dict of its kind (plan_activation_memory; planned before
         anything is allocated)."""
@@ -1321,11 +1351,11 @@ class FusedMMDiTBase(nn.Module):
         Mt, Mi = B * T, B * Limg
         M, S = Mt + Mi, T + Limg
         nbytes = lambda shape, dt: math.prod(shape) * dt.itemsize
-        ws.update(B=B, T=T, Limg=Limg, S=S, Mt=Mt, Mi=Mi, M=M)
+        ws.update(B=B, T=T, Limg=Limg, S=S, Mt=Mt, Mi=Mi, M=M, det=det)
         nblk = n_double + n_single
         nd = n_double if train else min(1, n_double)
         ns = n_single if train else min(1, n_single)
-        pre, post = self._fixed_entries(B, T, Limg, train, nblk, extra)
+        pre, post = self._fixed_entries(B, T, Limg, train, nblk, extra, det)
         kinds = [("dbl", l) for l in range(nd)] + [("sgl", l) for l in range(ns)]
         plan = ActivationPlan((), 0, 0, 0, None)
         if train:
@@ -1358,12 +1388,12 @@ class FusedMMDiTBase(nn.Module):
         return ws
 
     def _get_workspace(self, key, build):
-        """key = (B, T, Limg, train).  One training workspace (tens of GB of saved activations) and up to three inference workspaces
+        """key = (B, T, Limg, train, det), det: torch.are_deterministic_algorithms_enabled() of a training forward.  One training workspace (tens of GB of saved activations) and up to three inference workspaces
         (a few hundred MB each: validation alternates between the prompt and the negative prompt, whose text lengths may differ) stay
         allocated, so switching between them neither re-allocates nor invalidates the CUDA graphs captured on them."""
         if self._ws_key == key:
             return self._ws
-        train = bool(key[-1])
+        train = bool(key[3])
         cached = self._train_ws if train else self._infer_ws.get(key)
         if cached is not None and (not train or cached[0] == key):
             ws = cached[1] if train else cached
@@ -1414,7 +1444,7 @@ class GraphCache:
         """fn(*args) through the graph of key (input signature, tag)."""
         if not enabled or self.failed or model._sharded is not None or model.dev.type != "cuda" or not torch.cuda.is_available():
             return fn(*args)
-        key = (_graph_sig(args), tag)
+        key = (_graph_sig(args), tag, torch.are_deterministic_algorithms_enabled())  # never replay across the two kernel choices
         ent = self.entries.pop(key, None)
         if ent is None:
             while len(self.entries) >= self.capacity:

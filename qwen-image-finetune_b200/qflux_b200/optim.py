@@ -30,6 +30,7 @@ class FusedLoraAdamW(torch.optim.Optimizer):
         self.exp_avg = torch.zeros(n, device=model.dev, dtype=torch.float32)
         self.exp_avg_sq = torch.zeros(n, device=model.dev, dtype=torch.float32)
         self.grad_norm_sq = torch.zeros(1, device=model.dev, dtype=torch.float32)
+        self._norm_parts = torch.zeros(lib.DET_NORM_PARTIALS, device=model.dev, dtype=torch.float32)  # deterministic norm
         members = []
         for full, pA, pB, ga, gb, d_in, d_out in model._all_members():
             members += [(pA.data, ga), (pB.data, gb)]
@@ -48,8 +49,12 @@ class FusedLoraAdamW(torch.optim.Optimizer):
         div = grad_divisor if grad_divisor is not None else self.grad_divisor
         g = self.param_groups[0]
         self.step_count += 1
-        lib.fused_adamw(self._tables, self.model.G32, self.exp_avg, self.exp_avg_sq, self.grad_norm_sq, 1.0 / float(div),
-                        self.max_grad_norm, g["lr"], g["betas"][0], g["betas"][1], g["eps"], g["weight_decay"], self.step_count)
+        args = (self._tables, self.model.G32, self.exp_avg, self.exp_avg_sq, self.grad_norm_sq, 1.0 / float(div), self.max_grad_norm,
+                g["lr"], g["betas"][0], g["betas"][1], g["eps"], g["weight_decay"], self.step_count)
+        if torch.are_deterministic_algorithms_enabled():  # the clip's norm summed in a fixed order: bit-reproducible
+            lib.fused_adamw_det(*args, scratch=self._norm_parts)
+        else:
+            lib.fused_adamw(*args)
         return loss
 
     def zero_grad(self, set_to_none: bool = True):

@@ -135,7 +135,9 @@ class QwenImageB200(FusedMMDiTBase):
         D = self.D
         extra = [("sin", (B, 256)), ("t1", (B, D)), ("temb", (B, D)), ("mods", (B, self.L * 2 * 6 * D)), ("fmod", (B, 2 * D)),
                  ("txt_n", (B * T, self.J))]
-        return self._get_workspace((B, T, Limg, train), lambda: self._alloc_common({}, B, T, Limg, train, self.L, extra=extra))
+        det = train and torch.are_deterministic_algorithms_enabled()  # read on every forward: selects the fixed-order backward
+        return self._get_workspace((B, T, Limg, train, det),
+                                   lambda: self._alloc_common({}, B, T, Limg, train, self.L, extra=extra, det=det))
 
     def _rope(self, img_shapes, T):
         key = (tuple(tuple(s) for s in img_shapes), T)

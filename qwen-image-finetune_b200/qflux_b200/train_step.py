@@ -93,7 +93,10 @@ class _FusedStep:
         this micro-step accumulates).  Returns the loss (a workspace scalar)."""
         m = self.dit
         ws = m._ws
-        lib.flow_loss(pred, x0, noise, w, norm, ws["loss"], ws["dpred"])
+        if ws["det"]:
+            lib.flow_loss_det(pred, x0, noise, w, norm, ws["loss"], ws["dpred"], scratch=ws["det_scratch"])
+        else:
+            lib.flow_loss(pred, x0, noise, w, norm, ws["loss"], ws["dpred"])
         if not self._accumulating:
             m.G32.zero_()
         m._backward_impl(ws["dpred"])
