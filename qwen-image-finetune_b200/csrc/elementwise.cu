@@ -983,6 +983,7 @@ extern "C" int qfx_attn_delta(const void* O, int64_t ldo, const void* dO, int64_
 
 extern "C" int qfx_grad_finalize(const float* g, int64_t n, float pre_scale, float max_norm, float* sumsq, void* out_bf16,
                                  void* stream) {
+  QFX_CHECK_ARG(g && n > 0 && sumsq && out_bf16, "qfx_grad_finalize: bad arguments");
   QFX_CUDA(cudaMemsetAsync(sumsq, 0, sizeof(float), (cudaStream_t)stream));
   sumsq_kernel<<<592, 256, 0, (cudaStream_t)stream>>>(g, n, pre_scale, sumsq);
   clip_cast_kernel<<<592, 256, 0, (cudaStream_t)stream>>>(g, n, pre_scale, sumsq, max_norm, (bf16*)out_bf16);

@@ -238,7 +238,7 @@ extern "C" int qfx_fused_prodigy(const qfx_adamw_tensor* tensors_dev, const int*
 extern "C" int qfx_fused_adamw(const qfx_adamw_tensor* tensors_dev, const int* chunks_dev, int n_chunks, const float* grad,
                                int64_t n_grad, float* exp_avg, float* exp_avg_sq, float* sumsq, float pre_scale, float max_norm,
                                float lr, float beta1, float beta2, float eps, float weight_decay, int step, void* stream) {
-  QFX_CHECK_ARG(tensors_dev && chunks_dev && n_chunks > 0 && grad && exp_avg && exp_avg_sq && sumsq && step >= 1,
+  QFX_CHECK_ARG(tensors_dev && chunks_dev && n_chunks > 0 && grad && n_grad > 0 && exp_avg && exp_avg_sq && sumsq && step >= 1,
                 "qfx_fused_adamw: bad arguments");
   cudaStream_t st = (cudaStream_t)stream;
   QFX_CUDA(cudaMemsetAsync(sumsq, 0, sizeof(float), st));
@@ -257,7 +257,7 @@ extern "C" int qfx_fused_adamw_det(const qfx_adamw_tensor* tensors_dev, const in
                                    int64_t n_grad, float* exp_avg, float* exp_avg_sq, float* sumsq, float pre_scale, float max_norm,
                                    float lr, float beta1, float beta2, float eps, float weight_decay, int step, float* scratch,
                                    int64_t scratch_floats, void* stream) {
-  QFX_CHECK_ARG(tensors_dev && chunks_dev && n_chunks > 0 && grad && exp_avg && exp_avg_sq && sumsq && step >= 1,
+  QFX_CHECK_ARG(tensors_dev && chunks_dev && n_chunks > 0 && grad && n_grad > 0 && exp_avg && exp_avg_sq && sumsq && step >= 1,
                 "qfx_fused_adamw_det: bad arguments");
   QFX_CHECK_ARG(scratch && scratch_floats >= QFX_DET_NORM_PARTIALS, "qfx_fused_adamw_det: scratch holds %lld floats, needs %d",
                 (long long)scratch_floats, QFX_DET_NORM_PARTIALS);

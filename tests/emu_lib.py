@@ -247,21 +247,25 @@ def adamw_tables(members, device):
 
 def fused_adamw(tables, grad, exp_avg, exp_avg_sq, sumsq, pre_scale, max_norm, lr, beta1, beta2, eps, weight_decay, step):
     members, _ = tables
+    # the C ABI takes the scalars as fp32 and forms 1 - beta, 1 - lr * wd and the bias corrections in fp32 (optimizer.cu)
+    f32 = lambda x: float(torch.tensor(x, dtype=torch.float32))
+    pre_scale, max_norm, lr, beta1, beta2, eps, weight_decay = (f32(x) for x in (pre_scale, max_norm, lr, beta1, beta2, eps, weight_decay))
     g = grad * pre_scale
     sumsq.copy_((g ** 2).sum().reshape(1))
     coef = 1.0
     if max_norm > 0:
         coef = min(1.0, max_norm / (float(sumsq.sqrt()) + 1e-6))
     g = g * coef
-    bc1, bc2 = 1 - beta1 ** step, 1 - beta2 ** step
+    bc1, bc2 = f32(1 - f32(beta1 ** step)), f32(1 - f32(beta2 ** step))
+    omb1, omb2, decay = f32(1 - beta1), f32(1 - beta2), f32(1 - lr * weight_decay)
     for p, off in members:
         n = p.numel()
         gi = g[off: off + n].view(p.shape)
         m, v = exp_avg[off: off + n].view(p.shape), exp_avg_sq[off: off + n].view(p.shape)
-        w = p.float() * (1 - lr * weight_decay)
-        m.mul_(beta1).add_(gi, alpha=1 - beta1)
-        v.mul_(beta2).addcmul_(gi, gi, value=1 - beta2)
-        p.copy_((w - (lr / bc1) * m / (v.sqrt() / bc2 ** 0.5 + eps)).to(BF))
+        w = p.float() * decay
+        m.mul_(beta1).add_(gi, alpha=omb1)
+        v.mul_(beta2).addcmul_(gi, gi, value=omb2)
+        p.copy_((w - (lr / bc1) * m / (v.sqrt() / f32(bc2 ** 0.5) + eps)).to(BF))
 
 
 def attn_delta(O, dO, delta, tokens_per_sample, s_offset, dO_joint=None):

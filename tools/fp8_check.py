@@ -8,8 +8,10 @@
                                            conversion bit for bit; time and bytes/s of the launch
   qwen_step_parity / flux_step_parity      a multi-block full-width training step (Qwen 6 blocks; FLUX 3 double + 3 single, YAML
                                            targets): the FP8 model and a bf16 model holding the upcast weights give the same
-                                           prediction bit for bit; loss and every LoRA gradient tensor are no further apart than two
-                                           runs of the same model are (the loss and some gradient sums are reduced with atomics)
+                                           prediction bit for bit; the loss and the whole LoRA gradient are no further apart than
+                                           two runs of the same model are (the loss and some gradient sums are reduced with atomics);
+                                           under torch.use_deterministic_algorithms(True) the loss and every LoRA gradient tensor
+                                           agree bit for bit
   graph_replay                             a CUDA-graph replayed FP8 training step equals its eager run (Qwen and FLUX)
   infer_replay                             the replayed FP8 inference forward is bit-exact and the graph cache captured
 """
@@ -149,23 +151,27 @@ def _step_parity(family, name, cfg):
     r = bf16_twin(m)
     r.add_adapter(cfg["r"], cfg["r"], target_modules=m.peft_config[m.adapter_name].target_modules, b_std=0.02)  # same seeded factors
     assert all(torch.equal(p, r._lora_params[k]) for k, p in m._lora_params.items())
+    # flag off (the default path): the forward is bit-identical; the loss and some gradient sums end in floating-point atomics, so
+    # two runs of one model differ, and the pooled FP8-vs-bf16 distance is held to that rerun spread
     a, a2 = nf4_check._one_step(m, family, batch), nf4_check._one_step(m, family, batch)
     b, b2 = nf4_check._one_step(r, family, batch), nf4_check._one_step(r, family, batch)
-    va, va2, vb, vb2 = (x.lora_grad_views(g[2]) for x, g in ((m, a), (m, a2), (r, b), (r, b2)))
-    worst, n_bitwise, fails = 0.0, 0, []
-    for k in vb:
-        d, noise = harness.rel_l2(va[k], vb[k]), max(harness.rel_l2(vb2[k], vb[k]), harness.rel_l2(va2[k], va[k]))
-        n_bitwise += bool(torch.equal(va[k], vb[k]))
-        worst = max(worst, d / (noise + 1e-12) if d > 0 else 0.0)
-        if d > 2 * noise + 1e-6:
-            fails.append((k, d, noise))
+    pooled, pooled_noise = harness.rel_l2(a[2], b[2]), max(harness.rel_l2(b2[2], b[2]), harness.rel_l2(a2[2], a[2]))
+    # flag on: every reduction in a fixed order, so the two models must agree bit for bit, loss and every LoRA gradient tensor
+    torch.use_deterministic_algorithms(True)
+    try:
+        da, db = nf4_check._one_step(m, family, batch), nf4_check._one_step(r, family, batch)
+    finally:
+        torch.use_deterministic_algorithms(False)
+    va, vb = m.lora_grad_views(da[2]), r.lora_grad_views(db[2])
+    differ = [k for k in vb if not torch.equal(va[k].view(torch.int32), vb[k].view(torch.int32))]
     res = dict(family=family, blocks=m.L + m.Ls, pred_identical=bool(torch.equal(a[1], b[1])), loss_fp8=a[0], loss_bf16=b[0],
-               loss_bf16_again=b2[0], lora_tensors=len(vb), bitwise_equal_tensors=n_bitwise,
-               bf16_rerun_bitwise=bool(torch.equal(b[2], b2[2])), grad_rel_fp8_vs_bf16=harness.rel_l2(a[2], b[2]),
-               grad_rel_bf16_vs_bf16=harness.rel_l2(b2[2], b[2]), worst_ratio_to_rerun_noise=round(worst, 3), fails=fails[:5],
-               gpu=torch.cuda.get_device_name())
+               loss_bf16_again=b2[0], lora_tensors=len(vb), bf16_rerun_bitwise=bool(torch.equal(b[2], b2[2])),
+               grad_rel_fp8_vs_bf16=pooled, grad_rel_rerun=pooled_noise,
+               det_pred_identical=bool(torch.equal(da[1], db[1])), det_loss_identical=da[0] == db[0],
+               det_differing_tensors=differ[:5], gpu=torch.cuda.get_device_name())
     print(res)
-    assert res["pred_identical"] and abs(a[0] - b[0]) <= 1e-6 * abs(b[0]) and not fails
+    assert res["pred_identical"] and abs(a[0] - b[0]) <= 1e-6 * abs(b[0]) and pooled <= 2 * pooled_noise + 1e-6
+    assert res["det_pred_identical"] and res["det_loss_identical"] and not differ
     return res
 
 
@@ -221,6 +227,9 @@ CASES = dict(kernel_all_codes=kernel_all_codes, kernel_qwen_double=kernel_qwen_d
              qwen_step_parity=qwen_step_parity, flux_step_parity=flux_step_parity, graph_replay=graph_replay, infer_replay=infer_replay)
 
 if __name__ == "__main__":
+    # the step-parity cases run a step under use_deterministic_algorithms(True), where torch allows the modulation-LoRA cuBLAS
+    # products only with a fixed workspace configuration (INTEGRATION.md); set before anything initialises cuBLAS here
+    os.environ.setdefault("CUBLAS_WORKSPACE_CONFIG", ":4096:8")
     if len(sys.argv) == 2 and sys.argv[1] in CASES:  # one case in this process (tests/test_fp8_weights.py)
         print(CASES[sys.argv[1]]())
     else:
