@@ -288,6 +288,38 @@ int qfx_fused_prodigy(const qfx_adamw_tensor* tensors, const int* chunks, int n_
                       double growth_rate, void* stream);
 
 /* ------------------------------------------------------------------------------------------------------------------
+ * Fused clip + 8-bit Adam over the flat fp32 LoRA gradient buffer: bitsandbytes' `optim.Adam8bit` (Optimizer2State "adam", block-wise,
+ * percentile_clipping 100, no amsgrad; csrc/kernels.cu kOptimizerStatic8bit2StateBlockwise and kOptimizer32bit2State) after the clip of
+ * qfx_fused_adamw, on the same `tensors` / `chunks` tables.  With g = grad * pre_scale * min(1, max_norm / (||grad*pre_scale|| + 1e-6))
+ * (max_norm <= 0: no clip), per element in the fp32 arithmetic of those kernels, with step t >= 1:
+ *   c1 = 1 - beta1^t,  c2 = sqrt(1 - beta2^t),  step_size = -lr c2 / c1                   (host, fp32)
+ *   s1 = s1 beta1 + (1 - beta1) g ;  s2 = s2 beta2 + (1 - beta2) g g
+ *   p = bf16(p + step_size s1 / (sqrt(s2) + c2 eps)) ;  p = bf16(p (1 - lr weight_decay))    (the second only when weight_decay > 0)
+ * A non-finite g leaves its parameter alone and sets both states to 0, as bitsandbytes does.  lr == 0 still updates the states.
+ * Tensor i (chunks' first member) keeps its states
+ *   - numel < min_8bit_size: fp32 s1 = s1_32[state_offsets[i] + e], s2 = s2_32[...]  (bitsandbytes' 32-bit path);
+ *   - otherwise 8-bit, block-wise: uint8 codes state1 / state2 at grad_offset + e (n_grad bytes each, like grad) and one fp32 absmax1 /
+ *     absmax2 per QFX_ADAM8BIT_BLOCK elements of the tensor at state_offsets[i] + e / QFX_ADAM8BIT_BLOCK (the last block may be partial).
+ *     Per block: the old states are qmap[code] * absmax_old; the new absmax is the block's max |s| over its elements; the parameter
+ *     takes the unquantized new states; the new code is the nearest entry of the sorted 256-entry map to s / absmax (a tie takes the
+ *     lower code).  state1 then follows bitsandbytes' sign rule: when qmap1[code] and s1 differ in sign bit, the code steps one
+ *     toward s1.  A block whose new absmax is 0 stores QFX_ADAM8BIT_CODE1_ZERO / QFX_ADAM8BIT_CODE2_ZERO (the maps' 0 entries).
+ *   qmap1 / qmap2: bitsandbytes' create_dynamic_map(signed=True) / (signed=False), 256 sorted fp32 values each (0 at index 127 / 0).
+ * Codes of fp32-path tensors are not touched.  sumsq receives ||grad*pre_scale||^2; the norm's QFX_DET_NORM_PARTIALS partials go
+ * to fp32 `scratch` (scratch_floats >= QFX_DET_NORM_PARTIALS) and are added in a fixed order.  Three launches on `stream`, no host
+ * synchronisation, no floating-point atomics: the same inputs give the same bits.
+ * QFX_ADAM8BIT_BLOCK follows bitsandbytes 0.45 and later, whose block-wise 8-bit optimizers use 256 (older releases used 2048);
+ * it divides QFX_ADAMW_CHUNK, so no block crosses a chunk. */
+#define QFX_ADAM8BIT_BLOCK 256
+#define QFX_ADAM8BIT_CODE1_ZERO 127
+#define QFX_ADAM8BIT_CODE2_ZERO 0
+int qfx_fused_adam8bit(const qfx_adamw_tensor* tensors, const int* chunks, int n_chunks, const int64_t* state_offsets, const float* grad,
+                       int64_t n_grad, unsigned char* state1, unsigned char* state2, float* absmax1, float* absmax2, float* s1_32,
+                       float* s2_32, const float* qmap1, const float* qmap2, float* sumsq, float* scratch, int64_t scratch_floats,
+                       float pre_scale, float max_norm, float lr, float beta1, float beta2, float eps, float weight_decay, int step,
+                       int min_8bit_size, void* stream);
+
+/* ------------------------------------------------------------------------------------------------------------------
  * NF4 frozen weights (4-bit base checkpoints: bitsandbytes `Linear4bit`, whose forward dequantizes the weight to bf16 and runs a
  * plain matmul, bitsandbytes/functional.py dequantize_4bit).  One launch dequantizes up to QFX_NF4_MAX_SEGMENTS tensors (the NF4
  * matrices of one block) into bf16:  out[i] = bf16_rn(NF4[nibble_i] * absmax[i / blocksize])  with the product in fp32,

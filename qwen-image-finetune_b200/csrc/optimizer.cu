@@ -7,6 +7,7 @@
 // the GEMMs read, so B factors are row-strided).  Moments are fp32 (torch keeps them in the parameter dtype, bf16).
 // The same tables drive the configs' other optimizer, prodigyopt.Prodigy (qfx_fused_prodigy): its two global sums (sum g*(p0-p) and
 // sum |s|) are per-CTA partials added in a fixed order on the device, where prodigyopt calls .item() twice per parameter tensor.
+// And bitsandbytes' block-wise Adam8bit (qfx_fused_adam8bit): one pass over the chunks with uint8 states and per-block absmax.
 #include <string.h>
 
 #include "../../include/qfx.h"
@@ -196,9 +197,137 @@ __global__ void __launch_bounds__(256) prodigy_pass_b_kernel(const qfx_adamw_ten
   }
 }
 
+// ---- 8-bit Adam (qfx.h qfx_fused_adam8bit).  The nearest entry of the sorted 256-entry map q (shared memory) to x; a tie takes the
+// lower code.  lo ends as the last index with q[lo] <= x (0 when x < q[0]).
+__device__ __forceinline__ int adam8bit_quantize(const float* q, float x) {
+  int lo = 0;
+#pragma unroll
+  for (int s = 128; s > 0; s >>= 1)
+    if (q[lo + s] <= x) lo += s;
+  return lo < 255 && x > 0.5f * (q[lo] + q[lo + 1]) ? lo + 1 : lo;
+}
+
+// One CTA per chunk.  Warp w takes the chunk's blocks w, w + 8 (QFX_ADAMW_CHUNK / QFX_ADAM8BIT_BLOCK = 16 of them), lane l the block's
+// elements l, l + 32, ..., so a block's absmax is one warp reduction and no block is split between warps.
+constexpr int kAdam8bitPerLane = QFX_ADAM8BIT_BLOCK / 32;
+static_assert(QFX_ADAMW_CHUNK % QFX_ADAM8BIT_BLOCK == 0, "a block must not cross a chunk");
+
+__global__ void __launch_bounds__(256) fused_adam8bit_kernel(const qfx_adamw_tensor* __restrict__ tensors, const int2* __restrict__ chunks,
+                                                             const int64_t* __restrict__ state_offsets, const float* __restrict__ g,
+                                                             uint8_t* __restrict__ code1, uint8_t* __restrict__ code2,
+                                                             float* __restrict__ absmax1, float* __restrict__ absmax2,
+                                                             float* __restrict__ s1_32, float* __restrict__ s2_32,
+                                                             const float* __restrict__ qmap1, const float* __restrict__ qmap2,
+                                                             const float* __restrict__ sumsq, float pre_scale, float max_norm, float beta1,
+                                                             float beta2, float c2eps, float step_size, float decay, int min_8bit_size) {
+  __shared__ float q1[256], q2[256];
+  q1[threadIdx.x] = qmap1[threadIdx.x];
+  q2[threadIdx.x] = qmap2[threadIdx.x];
+  __syncthreads();
+  const int2 ck = chunks[blockIdx.x];
+  const qfx_adamw_tensor t = tensors[ck.x];
+  const int64_t so = state_offsets[ck.x];
+  const bool blockwise = t.numel >= min_8bit_size;
+  float coef = pre_scale;
+  if (max_norm > 0.f) {
+    const float c = max_norm / (sqrtf(*sumsq) + 1e-6f);  // torch.nn.utils.clip_grad_norm_
+    coef *= c < 1.f ? c : 1.f;
+  }
+  bf16* p = reinterpret_cast<bf16*>(t.param);
+  const int end = min(t.numel, ck.y + QFX_ADAMW_CHUNK), lane = threadIdx.x & 31;
+  for (int b0 = ck.y + (threadIdx.x >> 5) * QFX_ADAM8BIT_BLOCK; b0 < end; b0 += 8 * QFX_ADAM8BIT_BLOCK) {
+    const int64_t blk = so + b0 / QFX_ADAM8BIT_BLOCK;
+    const float a1 = blockwise ? absmax1[blk] : 0.f, a2 = blockwise ? absmax2[blk] : 0.f;
+    float s1[kAdam8bitPerLane], s2[kAdam8bitPerLane], m1 = 0.f, m2 = 0.f;
+    unsigned finite = 0;  // bit j: element j of this lane has a finite gradient
+#pragma unroll
+    for (int j = 0; j < kAdam8bitPerLane; ++j) {
+      const int e = b0 + lane + 32 * j;
+      s1[j] = s2[j] = 0.f;
+      if (e >= end) continue;
+      const int64_t fi = t.grad_offset + e;
+      const float gi = g[fi] * coef;
+      if (!isfinite(gi)) continue;  // bitsandbytes: both states 0, the parameter untouched
+      finite |= 1u << j;
+      const float o1 = blockwise ? q1[code1[fi]] * a1 : s1_32[so + e];
+      const float o2 = blockwise ? q2[code2[fi]] * a2 : s2_32[so + e];
+      s1[j] = o1 * beta1 + (1.f - beta1) * gi;
+      // the 8-bit kernel forms (1 - beta2) g g left to right, the 32-bit kernel (1 - beta2) (g g)
+      s2[j] = blockwise ? o2 * beta2 + (1.f - beta2) * gi * gi : o2 * beta2 + (1.f - beta2) * (gi * gi);
+      m1 = fmaxf(m1, fabsf(s1[j]));
+      m2 = fmaxf(m2, fabsf(s2[j]));
+    }
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) {
+      m1 = fmaxf(m1, __shfl_xor_sync(0xffffffffu, m1, o));
+      m2 = fmaxf(m2, __shfl_xor_sync(0xffffffffu, m2, o));
+    }
+    if (blockwise && lane == 0) {
+      absmax1[blk] = m1;
+      absmax2[blk] = m2;
+    }
+#pragma unroll
+    for (int j = 0; j < kAdam8bitPerLane; ++j) {
+      const int e = b0 + lane + 32 * j;
+      if (e >= end) continue;
+      const int64_t fi = t.grad_offset + e;
+      const int row = e / t.cols, col = e - row * t.cols;
+      bf16* pp = p + (int64_t)row * t.ld + col;
+      if (finite >> j & 1) {
+        // decay is 1 without weight decay: the second rounding then returns the bf16 value unchanged
+        const bf16 w = __float2bfloat16_rn(__bfloat162float(*pp) + step_size * (s1[j] / (sqrtf(s2[j]) + c2eps)));
+        *pp = __float2bfloat16_rn(__bfloat162float(w) * decay);
+      }
+      if (!blockwise) {
+        s1_32[so + e] = s1[j];
+        s2_32[so + e] = s2[j];
+        continue;
+      }
+      int c1 = QFX_ADAM8BIT_CODE1_ZERO, c2 = QFX_ADAM8BIT_CODE2_ZERO;
+      if (m1 > 0.f) {
+        c1 = adam8bit_quantize(q1, s1[j] / m1);
+        if (signbit(q1[c1]) != signbit(s1[j])) c1 += s1[j] > 0.f ? 1 : -1;
+      }
+      if (m2 > 0.f) c2 = adam8bit_quantize(q2, s2[j] / m2);
+      code1[fi] = (uint8_t)c1;
+      code2[fi] = (uint8_t)c2;
+    }
+  }
+}
+
 }  // namespace qfx
 
 using namespace qfx;
+
+extern "C" int qfx_fused_adam8bit(const qfx_adamw_tensor* tensors_dev, const int* chunks_dev, int n_chunks, const int64_t* state_offsets,
+                                  const float* grad, int64_t n_grad, unsigned char* state1, unsigned char* state2, float* absmax1,
+                                  float* absmax2, float* s1_32, float* s2_32, const float* qmap1, const float* qmap2, float* sumsq,
+                                  float* scratch, int64_t scratch_floats, float pre_scale, float max_norm, float lr, float beta1,
+                                  float beta2, float eps, float weight_decay, int step, int min_8bit_size, void* stream) {
+  QFX_CHECK_ARG(tensors_dev && chunks_dev && n_chunks > 0 && state_offsets && grad && n_grad > 0 && state1 && state2 && absmax1 &&
+                    absmax2 && s1_32 && s2_32 && qmap1 && qmap2 && sumsq && step >= 1 && min_8bit_size >= 0,
+                "qfx_fused_adam8bit: bad arguments");
+  QFX_CHECK_ARG(scratch && scratch_floats >= QFX_DET_NORM_PARTIALS, "qfx_fused_adam8bit: scratch holds %lld floats, needs %d",
+                (long long)scratch_floats, QFX_DET_NORM_PARTIALS);
+  QFX_CHECK_ARG(lr >= 0.f, "qfx_fused_adam8bit: needs lr >= 0, got %g", (double)lr);
+  cudaStream_t st = (cudaStream_t)stream;
+  adamw_sumsq_kernel<true><<<QFX_DET_NORM_PARTIALS, 256, 0, st>>>(grad, n_grad, pre_scale, scratch);
+  QFX_CUDA(cudaGetLastError());
+  SplitSum S;
+  memset(&S, 0, sizeof(S));
+  S.part = scratch; S.split_stride = 1; S.splits = QFX_DET_NORM_PARTIALS; S.rows = S.cols = 1;
+  S.dst[0] = sumsq; S.rows_per_dst = S.cols_per_dst = 1; S.accumulate = 0;
+  int rc = launch_split_sum(S, st);
+  if (rc) return rc;
+  // bitsandbytes forms these in fp32 (kernels.cu: correction1, correction2, step_size; the decay factor 1 - lr * weight_decay)
+  const float c1 = 1.f - powf(beta1, (float)step), c2 = sqrtf(1.f - powf(beta2, (float)step));
+  const float step_size = -lr * c2 / c1, decay = weight_decay > 0.f ? 1.f - lr * weight_decay : 1.f;
+  fused_adam8bit_kernel<<<n_chunks, 256, 0, st>>>(tensors_dev, reinterpret_cast<const int2*>(chunks_dev), state_offsets, grad, state1,
+                                                  state2, absmax1, absmax2, s1_32, s2_32, qmap1, qmap2, sumsq, pre_scale, max_norm, beta1,
+                                                  beta2, c2 * eps, step_size, decay, min_8bit_size);
+  QFX_CUDA(cudaGetLastError());
+  return 0;
+}
 
 extern "C" int qfx_fused_prodigy(const qfx_adamw_tensor* tensors_dev, const int* chunks_dev, int n_chunks, const float* grad,
                                  int64_t n_grad, float* exp_avg, float* exp_avg_sq, float* s, const void* p0, double* scalars,

@@ -26,7 +26,7 @@ class QfxError(RuntimeError):
 LAUNCHES = 0  # kernels of THIS library launched so far (bench.py reports the per-step delta as gpu_launches)
 _KERNELS_PER_CALL = {"qfx_grad_finalize": 2, "qfx_attn_bwd_det": 2, "qfx_lora_wgrad_tc_det": 2, "qfx_lora_wgrad_det": 2,
                      "qfx_mod_grad_det": 2, "qfx_flow_loss_det": 2, "qfx_grad_finalize_det": 3, "qfx_fused_adamw_det": 3,
-                     "qfx_fused_prodigy": 5}
+                     "qfx_fused_prodigy": 5, "qfx_fused_adam8bit": 3}
 
 
 def check(rc: int, what: str):
@@ -410,6 +410,55 @@ def fused_prodigy(tables, grad, exp_avg, exp_avg_sq, s, p0, scalars, sumsq, scra
                    ptr(scalars), ptr(sumsq), *_scratch(scratch), float(pre_scale), float(max_norm), float(lr), float(beta1), float(beta2),
                    float(beta3), float(eps), float(weight_decay), int(bool(decouple)), int(bool(use_bias_correction)),
                    int(bool(safeguard_warmup)), float(d0), float(d_coef), float(growth_rate), cur_stream()), "qfx_fused_prodigy")
+
+
+# 8-bit Adam (qfx.h qfx_fused_adam8bit)
+ADAM8BIT_BLOCK = 256
+_adam8bit = _sig("qfx_fused_adam8bit", _vp, _vp, _i, _vp, _vp, _i64, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i64, _f, _f, _f, _f, _f,
+                 _f, _f, _i, _i, _vp)
+
+
+def dynamic_map(signed: bool):
+    """bitsandbytes' `functional.create_dynamic_map(signed)` with its defaults (7 exponent bits, 8 bits): 256 sorted fp32 values,
+    built the way bitsandbytes builds them (fp32 linspace means, scaled in Python floats)."""
+    data = []
+    for i in range(7):
+        items = 2 ** i + 1 if signed else 2 ** (i + 1) + 1
+        b = torch.linspace(0.1, 1, items, dtype=torch.float32)
+        means = (b[:-1] + b[1:]) / 2.0
+        data += ((10 ** (-6 + i)) * means).tolist()
+        if signed:
+            data += (-(10 ** (-6 + i)) * means).tolist()
+    data += [0, 1.0]
+    return torch.tensor(sorted(data), dtype=torch.float32)
+
+
+def adam8bit_layout(members, min_8bit_size):
+    """Per tensor of `members` ((param, grad offset) pairs, as adamw_tables takes them): the offset of its absmax blocks (numel >=
+    min_8bit_size) or of its fp32 states (smaller tensors), in member order.  Returns (offsets, absmax values, fp32 state elements)."""
+    offsets, n_absmax, n_small = [], 0, 0
+    for p, _ in members:
+        n = p.numel()
+        if n >= min_8bit_size:
+            offsets.append(n_absmax)
+            n_absmax += -(-n // ADAM8BIT_BLOCK)
+        else:
+            offsets.append(n_small)
+            n_small += n
+    return offsets, n_absmax, n_small
+
+
+def fused_adam8bit(tables, state_offsets, grad, state1, state2, absmax1, absmax2, s1_32, s2_32, qmap1, qmap2, sumsq, scratch, pre_scale,
+                   max_norm, lr, beta1, beta2, eps, weight_decay, step, min_8bit_size):
+    """Clip + one bitsandbytes Adam8bit step on every tensor of `tables` in place (qfx.h): fp32 grad, uint8 codes [n_grad], fp32 absmax
+    and small-tensor states at `state_offsets` (int64 device tensor, adam8bit_layout), fp32 maps [256]."""
+    raw, chunks = tables
+    require_cuda(raw, chunks, state_offsets, grad, state1, state2, absmax1, absmax2, s1_32, s2_32, qmap1, qmap2, sumsq, scratch)
+    assert state1.dtype == state2.dtype == torch.uint8 and state_offsets.dtype == torch.int64 and qmap1.numel() == qmap2.numel() == 256
+    check(_adam8bit(ptr(raw), ptr(chunks), chunks.shape[0], ptr(state_offsets), ptr(grad), grad.numel(), ptr(state1), ptr(state2),
+                    ptr(absmax1), ptr(absmax2), ptr(s1_32), ptr(s2_32), ptr(qmap1), ptr(qmap2), ptr(sumsq), *_scratch(scratch),
+                    float(pre_scale), float(max_norm), float(lr), float(beta1), float(beta2), float(eps), float(weight_decay), int(step),
+                    int(min_8bit_size), cur_stream()), "qfx_fused_adam8bit")
 
 
 def lora_wgrad(P, Q, G, gs_i, gs_j, r):

@@ -1,9 +1,9 @@
-"""Fused clip + optimizer step for the LoRA parameters of a fused MMDiT (SURVEY.md §8 f1): AdamW and Prodigy.
+"""Fused clip + optimizer step for the LoRA parameters of a fused MMDiT (SURVEY.md §8 f1): AdamW, Prodigy and 8-bit Adam.
 
 Mirrors what the reference's step body does after `accelerator.backward(loss)`
 (/root/reference/src/qflux/trainer/base_trainer.py:528-533): `clip_gradients()` (:449-455, global L2 norm over the trainable
 parameters, max_grad_norm) -> `optimizer.step()` (torch.optim.AdamW by default, :884-916 / config.py:534; prodigyopt.Prodigy in
-four of the shipped configs) -> `zero_grad()`.
+four of the shipped configs, bitsandbytes.optim.Adam8bit in eight) -> `zero_grad()`.
 The gradient is the model's flat fp32 accumulator (all-reduced by the caller for data parallel runs); nothing synchronises
 with the host.  Moments are kept in fp32 (torch keeps them in the parameter dtype, bf16) — documented deviation, DESIGN.md.
 """
@@ -87,6 +87,74 @@ class FusedLoraAdamW(FusedLoraOptimizer):
         self.step_count = int(fused["step"])
         self.exp_avg.copy_(fused["exp_avg"])
         self.exp_avg_sq.copy_(fused["exp_avg_sq"])
+
+
+class FusedLoraAdam8bit(FusedLoraOptimizer):
+    """bitsandbytes' `optim.Adam8bit` (block-wise 8-bit Adam) after the clip, as fused kernels over the flat gradient (qfx.h
+    qfx_fused_adam8bit): the constructor takes Adam8bit's arguments and defaults, plus `max_grad_norm`.  `optim_bits` is ignored
+    (Adam8bit always keeps 8-bit states) and so is `is_paged` (paging only decides where the state memory lives); `amsgrad`,
+    `percentile_clipping != 100`, `block_wise=False` and `args` are refused.  A step with lr == 0 still updates the states and the step
+    count, as in bitsandbytes.
+
+    State, per LoRA tensor in member order (A then B of each adapted Linear), laid out as bitsandbytes' per-parameter
+    `state1 / state2 / absmax1 / absmax2 / qmap1 / qmap2` concatenated:
+      * numel >= min_8bit_size: uint8 codes `state1[off: off + numel]`, `state2[...]` (off = the tensor's offset in the flat gradient,
+        row-major over the tensor) and fp32 `absmax1[a: a + ceil(numel / 256)]`, `absmax2[...]` (a = `state_offsets[i]`);
+      * smaller tensors: fp32 `s1_32[a: a + numel]`, `s2_32[...]`; their code bytes stay 0;
+      * `qmap1` / `qmap2`: the signed / unsigned dynamic maps, shared by every tensor (bitsandbytes keeps one copy per tensor).
+    `state_dict()` carries all of it and the step count."""
+
+    def __init__(self, model, lr: float = 1e-3, betas=(0.9, 0.999), eps: float = 1e-8, weight_decay: float = 0, amsgrad: bool = False,
+                 optim_bits: int = 32, args=None, min_8bit_size: int = 4096, percentile_clipping: int = 100, block_wise: bool = True,
+                 is_paged: bool = False, max_grad_norm: float = 1.0):
+        if amsgrad:
+            raise lib.QfxError("FusedLoraAdam8bit: amsgrad=True is not implemented")
+        if percentile_clipping != 100:
+            raise lib.QfxError(f"FusedLoraAdam8bit: percentile_clipping={percentile_clipping} is not implemented (it needs a 100-step "
+                               "history of gradient norms)")
+        if not block_wise:
+            raise lib.QfxError("FusedLoraAdam8bit: block_wise=False is not implemented (only block-wise 8-bit states)")
+        if args is not None:
+            raise lib.QfxError("FusedLoraAdam8bit: args (a bitsandbytes optimizer config object) is not supported; pass the arguments "
+                               "themselves")
+        super().__init__(model, dict(lr=lr, betas=tuple(betas), eps=eps, weight_decay=weight_decay), max_grad_norm)
+        self.min_8bit_size = int(min_8bit_size)
+        n, dev = model.G32.numel(), model.dev
+        offsets, n_absmax, n_small = lib.adam8bit_layout(self._members, self.min_8bit_size)
+        self.state_offsets = torch.tensor(offsets, dtype=torch.int64).to(dev)
+        self.state1 = torch.zeros(n, device=dev, dtype=torch.uint8)
+        self.state2 = torch.zeros(n, device=dev, dtype=torch.uint8)
+        self.absmax1 = torch.zeros(max(1, n_absmax), device=dev, dtype=torch.float32)  # one element when nothing is 8-bit: the C side
+        self.absmax2 = torch.zeros(max(1, n_absmax), device=dev, dtype=torch.float32)  # takes no null pointers
+        self.s1_32 = torch.zeros(max(1, n_small), device=dev, dtype=torch.float32)
+        self.s2_32 = torch.zeros(max(1, n_small), device=dev, dtype=torch.float32)
+        self.qmap1 = lib.dynamic_map(signed=True).to(dev)
+        self.qmap2 = lib.dynamic_map(signed=False).to(dev)
+        self.step_count = 0
+        self._norm_parts = torch.zeros(lib.DET_NORM_PARTIALS, device=dev, dtype=torch.float32)
+
+    _STATE = ("state1", "state2", "absmax1", "absmax2", "s1_32", "s2_32", "qmap1", "qmap2")
+
+    def _step(self, pre_scale):
+        g = self.param_groups[0]
+        self.step_count += 1
+        lib.fused_adam8bit(self._tables, self.state_offsets, self.model.G32, self.state1, self.state2, self.absmax1, self.absmax2,
+                           self.s1_32, self.s2_32, self.qmap1, self.qmap2, self.grad_norm_sq, self._norm_parts, pre_scale,
+                           self.max_grad_norm, g["lr"], g["betas"][0], g["betas"][1], g["eps"], g["weight_decay"], self.step_count,
+                           self.min_8bit_size)
+
+    def state_dict(self):
+        sd = super().state_dict()
+        sd["fused"] = dict(step=self.step_count, **{k: getattr(self, k) for k in self._STATE})
+        return sd
+
+    def load_state_dict(self, sd):
+        sd = dict(sd)
+        fused = sd.pop("fused")
+        super().load_state_dict(sd)
+        self.step_count = int(fused["step"])
+        for k in self._STATE:
+            getattr(self, k).copy_(fused[k])
 
 
 class FusedLoraProdigy(FusedLoraOptimizer):

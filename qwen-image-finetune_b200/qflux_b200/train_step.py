@@ -119,9 +119,10 @@ class _FusedStep:
 
 def _sync_and_step(dit, optimizer, max_grad_norm, micro_steps: int = 1):
     """Data-parallel tail of a step (base_trainer.py:383-388, 449-455, 528-533): ONE all-reduce(sum) of the flat fp32 LoRA
-    gradient, then either the fused clip + optimizer kernels (FusedLoraAdamW / FusedLoraProdigy read the accumulator directly; every
-    rank then holds the same gradient and parameters, so Prodigy's d agrees across ranks with no further collective) or, for any
-    torch optimizer, mean + clip + cast into the bf16 `.grad` views followed by `optimizer.step()`."""
+    gradient, then either the fused clip + optimizer kernels (FusedLoraAdamW / FusedLoraProdigy / FusedLoraAdam8bit read the
+    accumulator directly; every rank then holds the same gradient and parameters, so Prodigy's d and the 8-bit Adam states agree
+    across ranks with no further collective) or, for any torch optimizer, mean + clip + cast into the bf16 `.grad` views followed
+    by `optimizer.step()`."""
     from .optim import FusedLoraOptimizer
     world = 1
     if dist.is_available() and dist.is_initialized() and dist.get_world_size() > 1:
