@@ -122,9 +122,13 @@ int qfx_ln_modulate_bwd(const void* dy, int64_t lddy, const void* x, int64_t ldx
  * Linear carries LoRA):  per sample b (rows b*rows_per_batch ..) and column d, ACCUMULATED (+=) into fp32 [B, D] buffers:
  *   sum_out[b,d]  += sum_t g[t,d]                       (d shift; NULL to skip)
  *   prod_out[b,d] += sum_t g[t,d] * m[t,d]              (d scale with m = bf16(LN(x)) when mean/rstd are given (m = x),
- *                                                        d gate with m = the un-gated branch output when mean == NULL) */
+ *                                                        d gate with m = the un-gated branch output when mean == NULL)
+ * Refused before any CUDA call: M <= 0, D <= 0, D, ldg or ldm not a multiple of 8, M not a multiple of rows_per_batch > 0, and g or
+ * m not 16-byte aligned (both are read in 16-byte vectors).  qfx_mod_grad_det refuses the same. */
 int qfx_mod_grad(const void* g, int64_t ldg, const void* m, int64_t ldm, const float* mean, const float* rstd, int rows_per_batch,
                  float* sum_out, float* prod_out, int64_t ldo, int M, int D, void* stream);
+/* out = bf16(a * gate[b]).  a, gate and out are accessed in 16-byte vectors: D, lda, ldg and ldo must be multiples of 8 and the three
+ * bases 16-byte aligned, or the call is refused. */
 int qfx_gate_mul(const void* a, int64_t lda, const void* gate, int64_t ldg, int rows_per_batch, void* out, int64_t ldo, int M,
                  int D, void* stream);
 /* out = bf16(a + b), n elements (sums of the [B, D] conditioning embeddings, transformer_flux.py time_text_embed) */
@@ -178,10 +182,12 @@ int qfx_flow_noisy_input(const void* x0, const void* noise, const void* control,
 int qfx_flow_noisy_input_var(const void* x0, const void* noise, const void* control, const float* sigma, const int* Lt,
                              const int* Lc, void* packed, int B, int Ltmax, int Lcmax, int Ltot, int C, void* stream);
 /* loss = norm * sum_{b,t<L,c} w[b,t] (pred - (noise - x0))^2 ; dpred = d loss / d pred * grad_scale (zeros for t >= L)
- * — covers MseLoss / MaskEditLoss / AttentionMaskMseLoss (losses/*.py) through (w, norm). */
+ * — covers MseLoss / MaskEditLoss / AttentionMaskMseLoss (losses/*.py) through (w, norm).  loss is overwritten.  Refused unless
+ * loss != NULL, B, L, C > 0 and Ltot >= L (as qfx_flow_loss_det). */
 int qfx_flow_loss(const void* pred, const void* x0, const void* noise, const float* w, float norm, float grad_scale, float* loss,
                   void* dpred, int B, int L, int Ltot, int C, void* stream);
-/* G[i*gs_i + j*gs_j] += sum_m P[m,i] Q[m,j], j < r  (LoRA dB = dY^T (sXA^T), dA = (s dY B)^T X); fp32 atomics */
+/* G[i*gs_i + j*gs_j] += sum_m P[m,i] Q[m,j], j < r  (LoRA dB = dY^T (sXA^T), dA = (s dY B)^T X); fp32 atomics.
+ * Refused unless r is 4, 8, 16, 32 or 64, G != NULL, M > 0 and Dp > 0 (as qfx_lora_wgrad_det). */
 int qfx_lora_wgrad(const void* P, int64_t ldp, const void* Q, int64_t ldq, float* G, int64_t gs_i, int64_t gs_j, int M, int Dp,
                    int r, void* stream);
 /* The same LoRA weight gradients on the tensor cores (wgmma, both operands MN-major straight from HBM, rows split over CTAs,

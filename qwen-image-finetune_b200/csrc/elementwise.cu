@@ -806,9 +806,11 @@ extern "C" int qfx_ln_modulate_bwd(const void* dy, int64_t lddy, const void* x, 
 
 extern "C" int qfx_mod_grad(const void* g, int64_t ldg, const void* m, int64_t ldm, const float* mean, const float* rstd,
                             int rows_per_batch, float* sum_out, float* prod_out, int64_t ldo, int M, int D, void* stream) {
-  QFX_CHECK_ARG(D % 8 == 0 && ldg % 8 == 0 && (m == nullptr || ldm % 8 == 0) && rows_per_batch > 0 && M % rows_per_batch == 0,
+  QFX_CHECK_ARG(M > 0 && D > 0 && D % 8 == 0 && ldg % 8 == 0 && (m == nullptr || ldm % 8 == 0) && rows_per_batch > 0 &&
+                    M % rows_per_batch == 0,
                 "qfx_mod_grad: bad dims (D=%d, M=%d, rows_per_batch=%d)", D, M, rows_per_batch);
   QFX_CHECK_ARG((mean == nullptr) == (rstd == nullptr) && (mean == nullptr || m != nullptr), "qfx_mod_grad: mean/rstd need m");
+  QFX_CHECK_ARG(aligned(g, 16) && aligned(m, 16), "qfx_mod_grad: g / m must be 16-byte aligned");
   const int B = M / rows_per_batch, cb = (D + 255) / 256;
   int splits = (4 * num_sms() + cb * B - 1) / (cb * B);  // about four CTAs per SM
   splits = splits < 1 ? 1 : (splits > (rows_per_batch + 31) / 32 ? (rows_per_batch + 31) / 32 : splits);
@@ -820,6 +822,9 @@ extern "C" int qfx_mod_grad(const void* g, int64_t ldg, const void* m, int64_t l
 extern "C" int qfx_gate_mul(const void* a, int64_t lda, const void* gate, int64_t ldg, int rows_per_batch, void* out,
                             int64_t ldo, int M, int D, void* stream) {
   QFX_CHECK_ARG(D % 8 == 0, "qfx_gate_mul: D %% 8");
+  // a, gate and out are accessed in 16-byte vectors
+  QFX_CHECK_ARG(lda % 8 == 0 && ldg % 8 == 0 && ldo % 8 == 0, "qfx_gate_mul: leading dimensions must be multiples of 8 elements");
+  QFX_CHECK_ARG(aligned(a, 16) && aligned(gate, 16) && aligned(out, 16), "qfx_gate_mul: operands must be 16-byte aligned");
   gate_mul_kernel<<<(M + 7) / 8, 256, 0, (cudaStream_t)stream>>>((const bf16*)a, lda, (const bf16*)gate, ldg, rows_per_batch,
                                                                  (bf16*)out, ldo, M, D);
   LAUNCH_OK();
@@ -938,6 +943,7 @@ extern "C" int qfx_flow_noisy_input_var(const void* x0, const void* noise, const
 
 extern "C" int qfx_flow_loss(const void* pred, const void* x0, const void* noise, const float* w, float norm, float grad_scale,
                              float* loss, void* dpred, int B, int L, int Ltot, int C, void* stream) {
+  QFX_CHECK_ARG(loss && B > 0 && L > 0 && Ltot >= L && C > 0, "qfx_flow_loss: bad arguments");
   QFX_CUDA(cudaMemsetAsync(loss, 0, sizeof(float), (cudaStream_t)stream));
   flow_loss_kernel<<<296, 256, 0, (cudaStream_t)stream>>>((const bf16*)pred, (const bf16*)x0, (const bf16*)noise, w, norm,
                                                           grad_scale, loss, (bf16*)dpred, B, L, Ltot, C);
@@ -946,6 +952,8 @@ extern "C" int qfx_flow_loss(const void* pred, const void* x0, const void* noise
 
 extern "C" int qfx_lora_wgrad(const void* P, int64_t ldp, const void* Q, int64_t ldq, float* G, int64_t gs_i, int64_t gs_j,
                               int M, int Dp, int r, void* stream) {
+  QFX_CHECK_ARG(r == 4 || r == 8 || r == 16 || r == 32 || r == 64, "qfx_lora_wgrad: rank %d unsupported (4/8/16/32/64)", r);
+  QFX_CHECK_ARG(G && M > 0 && Dp > 0, "qfx_lora_wgrad: bad arguments");
   int splits = (M + 511) / 512;
   int rows = ((M + splits - 1) / splits + 63) / 64 * 64;
   dim3 grid((Dp + 127) / 128, (M + rows - 1) / rows);
@@ -1016,9 +1024,11 @@ extern "C" int qfx_zero_rows(void* out, int64_t ld, int ncols, const int* ranges
 extern "C" int qfx_mod_grad_det(const void* g, int64_t ldg, const void* m, int64_t ldm, const float* mean, const float* rstd,
                                 int rows_per_batch, float* sum_out, float* prod_out, int64_t ldo, int M, int D, float* scratch,
                                 int64_t scratch_floats, void* stream) {
-  QFX_CHECK_ARG(D % 8 == 0 && ldg % 8 == 0 && (m == nullptr || ldm % 8 == 0) && rows_per_batch > 0 && M % rows_per_batch == 0,
+  QFX_CHECK_ARG(M > 0 && D > 0 && D % 8 == 0 && ldg % 8 == 0 && (m == nullptr || ldm % 8 == 0) && rows_per_batch > 0 &&
+                    M % rows_per_batch == 0,
                 "qfx_mod_grad_det: bad dims (D=%d, M=%d, rows_per_batch=%d)", D, M, rows_per_batch);
   QFX_CHECK_ARG((mean == nullptr) == (rstd == nullptr) && (mean == nullptr || m != nullptr), "qfx_mod_grad_det: mean/rstd need m");
+  QFX_CHECK_ARG(aligned(g, 16) && aligned(m, 16), "qfx_mod_grad_det: g / m must be 16-byte aligned");
   const int B = M / rows_per_batch, cb = (D + 255) / 256;
   int splits = (QFX_DET_MODGRAD_CTAS + cb * B - 1) / (cb * B);
   splits = splits < 1 ? 1 : (splits > (rows_per_batch + 31) / 32 ? (rows_per_batch + 31) / 32 : splits);
