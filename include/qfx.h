@@ -367,6 +367,18 @@ int qfx_peer_open(const unsigned char* handle, void** ptr);
 int qfx_peer_close(void* ptr);
 int qfx_peer_copy_async(void* dst, const void* src, int64_t bytes, void* stream);
 
+/* ------------------------------------------------------------------------------------------------------------------
+ * Fixed-order sum of the ranks' flat fp32 LoRA gradients for bit-reproducible data-parallel steps on one node (replaces the
+ * all-reduce(sum) of the gradient under torch.use_deterministic_algorithms(True); qflux_b200/sharding.py GradExchange):
+ *   dst[i] = ((((+0) + src[0][i]) + src[1][i]) + ...) + src[nsrc-1][i]
+ * in source order, each add an IEEE fp32 round-to-nearest add with denormals kept and no fused multiply-add; the grid never changes
+ * the result.  A NaN result is some NaN (its payload is not specified).  `src` is a host array of nsrc <= QFX_MAX_RANKS device
+ * pointers: local allocations or peer mappings from qfx_peer_open.  dst may be one of the sources (the same pointer) but may not
+ * otherwise overlap one.  Every pointer 4-byte aligned; any n >= 0 (n == 0 launches nothing).  When all pointers share dst's
+ * offset modulo 16 bytes the bulk moves in 16-byte vectors.  One launch on `stream`, no host synchronisation. */
+#define QFX_MAX_RANKS 8
+int qfx_dp_reduce_det(const float* const* src, int nsrc, float* dst, int64_t n, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -708,3 +708,23 @@ def peer_close(p: int):
 def peer_copy_async(dst_ptr: int, src_ptr: int, nbytes: int, stream=None):
     s = cur_stream() if stream is None else C.c_void_p(stream.cuda_stream)
     _rc(_lib.qfx_peer_copy_async(C.c_void_p(dst_ptr), C.c_void_p(src_ptr), int(nbytes), s), "qfx_peer_copy_async")
+
+
+# ---------------------------------------------------------------------------------------------------- data-parallel sum (sharding.py)
+MAX_RANKS = 8
+_dp_reduce = _sig("qfx_dp_reduce_det", C.POINTER(C.c_void_p), _i, _vp, _i64, _vp)
+
+
+def dp_reduce_det(srcs, dst):
+    """dst = ((+0 + srcs[0]) + srcs[1]) + ... elementwise in fp32, in list order, bit-reproducible.  srcs: fp32 tensors of dst's
+    numel, or raw device pointers to that many floats (peer mappings); dst may be one of them, but may not otherwise overlap one."""
+    require_cuda(dst)
+    assert dst.dtype == torch.float32 and dst.is_contiguous() and 1 <= len(srcs) <= MAX_RANKS
+    ptrs = (C.c_void_p * len(srcs))()
+    for i, s in enumerate(srcs):
+        if torch.is_tensor(s):
+            require_cuda(s)
+            assert s.dtype == torch.float32 and s.is_contiguous() and s.numel() == dst.numel()
+            s = s.data_ptr()
+        ptrs[i] = s
+    check(_dp_reduce(ptrs, len(srcs), ptr(dst), dst.numel(), cur_stream()), "qfx_dp_reduce_det")

@@ -220,6 +220,7 @@ class FusedMMDiTBase(nn.Module):
         self.gradient_checkpointing = False  # accepted for interface compatibility (see enable_gradient_checkpointing)
         self._activation_limit = None  # bytes the training workspace may take; None: free device memory - ACTIVATION_HEADROOM
         self._sharded = None     # sharding.ShardedBlocks once shard_frozen_weights() has run (weights sharded across ranks)
+        self._grad_exchange = None  # sharding.GradExchange of deterministic data-parallel steps (False: ranks not on one host)
         self._bands_cache = {}   # (valid image rows per sample, Limg) -> lib.RowBands (ragged GEMM row bands)
         self._infer_graphs, self.use_cuda_graph_inference = GraphCache(8, "the inference forward"), True  # see _infer
         self._fwd_gen = 0        # bumped by every forward: autograd nodes of an older forward refuse to run (their activations are gone)
@@ -871,6 +872,17 @@ class FusedMMDiTBase(nn.Module):
         self.bind_param_grads()
         return self._gnorm_sq
 
+    def close(self):
+        """Teardown of a data-parallel run: unmap the memory this model maps from the other ranks (the deterministic gradient exchange's
+        peer gradients, then the sharded frozen weights' peer shards).  Collective when either exists: every rank must call it.  G32
+        moves back into an ordinary allocation; a model with sharded weights cannot run afterwards."""
+        if self._grad_exchange:
+            self._grad_exchange.close()
+        self._grad_exchange = None
+        for ring in (self._sharded, self._sharded_s):
+            if ring is not None:
+                ring.close()
+
     # ------------------------------------------------------------------------------------------------ helpers
     def _rows(self, ws, t, s):
         """rows of a stream-major [M, *] tensor: s=1 text, s=0 image."""
@@ -1454,6 +1466,8 @@ class GraphCache:
         self.entries[key] = ent
         if ent != "warm" and ent["ws"] is not model._ws and not model._activate_ws(ent["ws"], ent["ws_key"]):
             ent = "warm"  # the model dropped the workspace this graph was recorded on (another shape ran in between): record again
+        if ent != "warm" and ent["grad_ptr"] != _grad_ptr(model):
+            ent = "warm"  # the gradient accumulator moved (into peer memory, sharding.GradExchange): record again
         if ent == "warm":
             static = _graph_clone(args)
             torch.cuda.synchronize()
@@ -1471,7 +1485,7 @@ class GraphCache:
             # `keep`: per-shape tables the captured kernels point at (RoPE, key lengths, ragged row bands) live in bounded caches of the
             # model — the graph must keep them alive after they are evicted there
             ent = dict(graph=g, static=static, out=out, launches=lib.LAUNCHES - n0, ws=model._ws, ws_key=model._ws_key,
-                       keep=tuple(model._ws.get(k) for k in ("rope", "kv_len", "txt_len", "bands")))
+                       grad_ptr=_grad_ptr(model), keep=tuple(model._ws.get(k) for k in ("rope", "kv_len", "txt_len", "bands")))
             lib.LAUNCHES = n0  # capture launches nothing
             self.entries[key] = ent
         _graph_copy(ent["static"], args)
@@ -1479,6 +1493,11 @@ class GraphCache:
         lib.LAUNCHES += ent["launches"]
         model._fwd_gen += 1  # a replay is a forward that bypasses _forward_impl: autograd nodes of older forwards must refuse to run
         return ent["out"]
+
+
+def _grad_ptr(model):
+    g = getattr(model, "G32", None)  # None before an adapter exists
+    return 0 if g is None else g.data_ptr()
 
 
 def _graph_sig(a):

@@ -218,6 +218,119 @@ class ShardedBlocks(BlockRing):
             self._peer_buf.free()
 
 
+class GradExchange:
+    """Bit-reproducible data-parallel sum of the flat fp32 LoRA gradient `G32`: what `train_step._sync_and_step` runs in place of
+    `all_reduce(G32)` under torch.use_deterministic_algorithms(True) when every rank is a CUDA device of this host.  Element i of the
+    result is ((((+0) + g_0[i]) + g_1[i]) + ...) + g_{W-1}[i] in rank order (qfx_dp_reduce_det), the same bits on every rank:
+
+      1. reduce-scatter: rank q sums slice q of every rank's G32, read in place through CUDA IPC, into slice q of its own G32;
+      2. all-gather: rank q pulls every other rank's reduced slice with the copy engines, starting at the next rank.
+
+    Each rank moves 2 (W - 1) / W of the buffer, as a ring all-reduce does.  Nothing is allocated per step: the first exchange moves
+    G32 itself into an IPC-exportable allocation.  Three points order the ranks' streams: before the reduce (every G32 is final),
+    before the gather (every slice is reduced) and after it (every peer has pulled this rank's slices, so the next backward may write
+    G32 again).  At each, every rank records an interprocess CUDA event, a barrier on a gloo group guarantees that every rank has issued
+    its record, and the stream waits for the peers' events: the host never waits for the device and no kernel waits for another process.
+
+    CPU models (the emulated kernels of the gloo tests) run the same two phases with dist.all_gather in place of the peer reads."""
+
+    @staticmethod
+    def for_model(model):
+        """The model's exchange, set up by its first call (collective); None when the ranks are not all on this host with the same
+        kind of device."""
+        ex = getattr(model, "_grad_exchange", None)
+        if ex is None:
+            import socket
+            where = [None] * dist.get_world_size()
+            dist.all_gather_object(where, (socket.gethostname(), model.dev.type))
+            ex = model._grad_exchange = GradExchange(model) if len(set(where)) == 1 else False
+        return ex or None
+
+    def __init__(self, model):
+        self.model, self.dev, self.cuda = model, model.dev, model.dev.type == "cuda"
+        self.world, self.rank = dist.get_world_size(), dist.get_rank()
+        self.host = dist.group.WORLD if dist.get_backend() == "gloo" else dist.new_group(backend="gloo")
+        n = model.G32.numel()
+        c = -(-n // (self.world * ALIGN)) * ALIGN  # slice q = [q c, (q + 1) c), 512-byte aligned (the last may be short or empty)
+        self.bounds = [(min(n, q * c), min(n, (q + 1) * c)) for q in range(self.world)]
+        self._buf = None
+        if self.cuda:
+            self._open()
+
+    def _open(self):
+        from . import lib
+        with torch.cuda.device(self.dev):
+            self._buf = lib.PeerBuffer(self.model.G32.numel() * 4, self.dev)
+            g32 = self._buf.tensor(torch.float32, (self.model.G32.numel(),))
+            g32.copy_(self.model.G32)
+            self.model.G32 = g32
+            torch.cuda.empty_cache()  # the old accumulator's memory goes back to the device
+            self._events = [torch.cuda.Event(interprocess=True) for _ in range(3)]  # G32 final, slice reduced, peers' slices pulled
+            for e in self._events:
+                e.record()
+            mine = (self._buf.handle, [e.ipc_handle() for e in self._events])
+            peers = [None] * self.world
+            dist.all_gather_object(peers, mine, group=self.host)
+            self._ptrs = [self._buf.ptr if r == self.rank else lib.peer_open(peers[r][0], self.dev) for r in range(self.world)]
+            self._peer_events = [[torch.cuda.Event.from_ipc_handle(self.dev, h) for h in peers[r][1]]
+                                 for r in range(self.world) if r != self.rank]
+        dist.barrier(group=self.host)
+
+    def _point(self, k: int):
+        s = torch.cuda.current_stream(self.dev)
+        self._events[k].record(s)
+        dist.barrier(group=self.host)  # every rank has issued its record k: the waits below see this step's
+        for evs in self._peer_events:
+            s.wait_event(evs[k])
+
+    def all_reduce(self):
+        """G32 <- the rank-ordered sum of every rank's G32 (collective; asynchronous on the current stream)."""
+        from . import lib
+        g32 = self.model.G32
+        if not self.cuda:
+            bufs = [torch.empty_like(g32) for _ in range(self.world)]
+            dist.all_gather(bufs, g32, group=self.host)
+            lo, hi = self.bounds[self.rank]
+            if hi > lo:
+                lib.dp_reduce_det([b[lo:hi] for b in bufs], g32[lo:hi])
+            dist.all_gather(bufs, g32, group=self.host)
+            for r, (lo, hi) in enumerate(self.bounds):
+                if r != self.rank:
+                    g32[lo:hi] = bufs[r][lo:hi]
+            return
+        if g32.data_ptr() != self._buf.ptr:
+            raise RuntimeError("GradExchange: the model's G32 was replaced after the exchange was set up (add_adapter during "
+                               "data-parallel training); call model.close() on every rank first")
+        with torch.cuda.device(self.dev):
+            self._point(0)
+            lo, hi = self.bounds[self.rank]
+            if hi > lo:
+                lib.dp_reduce_det([p + lo * 4 for p in self._ptrs], g32[lo:hi])
+            self._point(1)
+            for i in range(1, self.world):
+                r = (self.rank + i) % self.world
+                lo, hi = self.bounds[r]
+                if hi > lo:
+                    lib.peer_copy_async(self._buf.ptr + lo * 4, self._ptrs[r] + lo * 4, (hi - lo) * 4)
+            self._point(2)
+
+    def close(self):
+        """Unmap the peers' gradients and move G32 back into an ordinary allocation (collective: every rank must call it)."""
+        if self._buf is None:
+            return
+        from . import lib
+        with torch.cuda.device(self.dev):
+            g32 = self.model.G32.clone()
+            torch.cuda.synchronize(self.dev)  # the last exchange's reads of the peers' memory have finished
+            for r, p in enumerate(self._ptrs):
+                if r != self.rank:
+                    lib.peer_close(p)
+            dist.barrier(group=self.host)
+            self.model.G32 = g32
+            self._buf.free()
+            self._buf = None
+
+
 class Nf4Blocks(BlockRing):
     """NF4-resident frozen weights: every NF4 matrix of a block kind lives as layer-stacked codes + fp32 absmax (nf4.py); a block's
     bf16 matrices are produced in its ring slot by ONE qfx_nf4_dequant launch right before it runs.  Kernels read the same

@@ -119,15 +119,21 @@ class _FusedStep:
 
 def _sync_and_step(dit, optimizer, max_grad_norm, micro_steps: int = 1):
     """Data-parallel tail of a step (base_trainer.py:383-388, 449-455, 528-533): ONE all-reduce(sum) of the flat fp32 LoRA
-    gradient, then either the fused clip + optimizer kernels (FusedLoraAdamW / FusedLoraProdigy / FusedLoraAdam8bit read the
+    gradient — under torch.use_deterministic_algorithms(True) with every rank on this host, the fixed-rank-order sum through peer
+    memory of sharding.GradExchange (bit-reproducible), else NCCL's — then either the fused clip + optimizer kernels (FusedLoraAdamW / FusedLoraProdigy / FusedLoraAdam8bit read the
     accumulator directly; every rank then holds the same gradient and parameters, so Prodigy's d and the 8-bit Adam states agree
     across ranks with no further collective) or, for any torch optimizer, mean + clip + cast into the bf16 `.grad` views followed
     by `optimizer.step()`."""
     from .optim import FusedLoraOptimizer
+    from .sharding import GradExchange
     world = 1
     if dist.is_available() and dist.is_initialized() and dist.get_world_size() > 1:
         world = dist.get_world_size()
-        dist.all_reduce(dit.G32)
+        exchange = GradExchange.for_model(dit) if torch.are_deterministic_algorithms_enabled() else None
+        if exchange is not None:
+            exchange.all_reduce()
+        else:
+            dist.all_reduce(dit.G32)
     inner = getattr(optimizer, "optimizer", optimizer)  # accelerate hands the trainer an AcceleratedOptimizer wrapper (.optimizer)
     if isinstance(inner, FusedLoraOptimizer):
         inner.max_grad_norm = max_grad_norm
