@@ -33,7 +33,8 @@ int qfx_version(void);
  *   trans_b = 1 :  out[M,N] = epi( alpha * ( A[M,K] . B[K,N]    +  A2[M,64*kb2] . B2[64*kb2,N]   ) )      (dgrad)
  *
  * The LoRA factor pair (A2,B2) is appended to the K loop of the SAME tensor-core contraction (rank padded to a
- * multiple of 64 with zeros by the caller), so one register accumulator receives base + low-rank update.
+ * multiple of 64 with zeros by the caller: kb2 = 1 for r <= 64, 2 for r <= 128, n times that for an n-slot dgrad), so one register
+ * accumulator receives base + low-rank update.
  * alpha scales the accumulator for the BIAS, ADD, DGELU and ATTN_DO epilogues only; GELU and RESID_GATE refuse alpha != 1.
  * out, out2, bias, resid, gate and aux are accessed as 16-byte vectors: their bases must be 16-byte aligned and their leading
  * dimensions multiples of 8 elements.
@@ -191,10 +192,11 @@ int qfx_flow_loss(const void* pred, const void* x0, const void* noise, const flo
 int qfx_lora_wgrad(const void* P, int64_t ldp, const void* Q, int64_t ldq, float* G, int64_t gs_i, int64_t gs_j, int M, int Dp,
                    int r, void* stream);
 /* The same LoRA weight gradients on the tensor cores (wgmma, both operands MN-major straight from HBM, rows split over CTAs,
- * fp32 atomics).  A [M, Na] (lda), B [M, 64*G] (ldb), both bf16 row-major; Gp: G device pointers to fp32 gradients.
- *   mode 0: for every group g < G and j < r:  Gp[g][i*gs_i + j*gs_j] += sum_m A[m,i] * B[m, g*64 + j]            (dA, or 1-group dB)
- *   mode 1 (Na = G*Dg): Gp[g][(i - g*Dg)*gs_i + j*gs_j] += sum_m A[m,i] * B[m, g*64 + j]  for g = i / Dg   (dB of a fused q|k|v site)
- * Na % 128 == 0. */
+ * fp32 atomics), 1 <= r <= 128.  A [M, Na] (lda), B [M, Rp*G] (ldb), both bf16 row-major, with Rp = 64 * ceil(r / 64) (64 or 128:
+ * each group's columns are the LoRA rank padded to whole 64-wide k-blocks); Gp: G device pointers to fp32 gradients.
+ *   mode 0: for every group g < G and j < r:  Gp[g][i*gs_i + j*gs_j] += sum_m A[m,i] * B[m, g*Rp + j]            (dA, or 1-group dB)
+ *   mode 1 (Na = G*Dg): Gp[g][(i - g*Dg)*gs_i + j*gs_j] += sum_m A[m,i] * B[m, g*Rp + j]  for g = i / Dg   (dB of a fused q|k|v site)
+ * Na % 128 == 0.  Each 64-wide rank chunk of the groups is its own CTA column (grid z), so A is read once per chunk. */
 int qfx_lora_wgrad_tc(const void* A, int64_t lda, int Na, const void* B, int64_t ldb, int G, int M, int mode, int Dg,
                       float* const* Gp, int64_t gs_i, int64_t gs_j, int r, void* stream);
 /* out = bf16(g * pre_scale * min(1, max_norm / (||g * pre_scale|| + 1e-6)))  (clip_grad_norm_, base_trainer.py:449-455);
@@ -233,9 +235,10 @@ int qfx_fused_adamw(const qfx_adamw_tensor* tensors, const int* chunks, int n_ch
 int qfx_attn_bwd_det(const void* Q, const void* K, const void* V, const void* dO, const float* lse, const float* delta,
                      float* dQ_accum, void* dK, void* dV, const int* kv_len, const int* txt_len, int split, int B, int H, int S,
                      float softmax_scale, void* stream);
-/* qfx_lora_wgrad_tc_det: qfx_lora_wgrad_tc.  With NG = (mode == 1 ? 1 : G) and tiles = Na / 128:
+/* qfx_lora_wgrad_tc_det: qfx_lora_wgrad_tc (1 <= r <= 128).  With NG = (mode == 1 ? 1 : G) and tiles = Na / 128:
  *   splits = max(1, min(ceil(M / 256), ceil(QFX_DET_WGRAD_CTAS / tiles))),  rows = 64 * ceil(ceil(M / splits) / 64),
- *   scratch_floats >= ceil(M / rows) * Na * NG * r            (at most ~QFX_DET_WGRAD_CTAS partial tiles of 128 x NG*r). */
+ *   scratch_floats >= ceil(M / rows) * Na * NG * r            (at most ~QFX_DET_WGRAD_CTAS partial tiles of 128 x NG*r).
+ * The split count does not depend on r: for r > 64 each split's two rank chunks store disjoint columns of the same partial tile. */
 #define QFX_DET_WGRAD_CTAS 264
 int qfx_lora_wgrad_tc_det(const void* A, int64_t lda, int Na, const void* B, int64_t ldb, int G, int M, int mode, int Dg,
                           float* const* Gp, int64_t gs_i, int64_t gs_j, int r, float* scratch, int64_t scratch_floats, void* stream);

@@ -195,8 +195,8 @@ class FluxB200(FusedMMDiTBase):
         for s in (0, 1):
             dYs = self._rows(ws, ws["dY"], s)
             lb = lbs[s]
-            ka = dict(A2=lb[0], B2=lb[1][:, :D], kb2=1) if lb is not None else {}
-            km = dict(A2=lb[0], B2=lb[1][:, D:], kb2=1) if lb is not None else {}
+            ka = dict(A2=lb[0], B2=lb[1][:, :D], kb2=lb[2]) if lb is not None else {}
+            km = dict(A2=lb[0], B2=lb[1][:, D:], kb2=lb[2]) if lb is not None else {}
             pa.append((dYs, Wo[:, :D], ka))
             pm.append(lib.gemm_problem(dYs, Wo[:, D:], self._rows(ws, ws["dbig"], s), aux=self._rows(ws, u, s),
                                        row_bands=self._bands(ws, s), **km))

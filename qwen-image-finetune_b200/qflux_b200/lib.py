@@ -472,8 +472,9 @@ _wgrad_tc = _sig("qfx_lora_wgrad_tc", _vp, _i64, _i, _vp, _i64, _i, _i, _i, _i, 
 
 
 def lora_wgrad_tc(A, B, G_list, gs_i, gs_j, r, mode=0, Dg=0):
-    """wgmma LoRA weight gradient: G_g += A^T B_g over rows.  A [M, Na], B [M, 64*G] bf16; G_list: fp32 tensors (one per
-    group).  mode 0: all A columns pair with every group; mode 1: A columns [g*Dg, (g+1)*Dg) pair with group g only."""
+    """wgmma LoRA weight gradient: G_g += A^T B_g over rows, r <= 128.  A [M, Na], B [M, Rp*G] bf16 with Rp = 64 * ceil(r / 64), group
+    g's columns [g*Rp, g*Rp + r); G_list: fp32 tensors (one per group).  mode 0: all A columns pair with every group; mode 1: A columns
+    [g*Dg, (g+1)*Dg) pair with group g only."""
     require_cuda(A, B, *G_list)
     n = len(G_list)
     arr = (C.c_void_p * n)(*[g.data_ptr() for g in G_list])
@@ -525,7 +526,8 @@ def _cdiv(a, b):
 
 
 def det_scratch_wgrad_tc(M, Na, ng, r):
-    """fp32 scratch of qfx_lora_wgrad_tc_det; ng = 1 for mode 1, else the number of groups."""
+    """fp32 scratch of qfx_lora_wgrad_tc_det; ng = 1 for mode 1, else the number of groups.  The split count does not depend on r,
+    so for r > 64 (two 64-wide rank chunks per group, each its own CTA) the rule is the same: splits x Na x ng x r floats."""
     splits = max(1, min(_cdiv(M, 256), _cdiv(DET_WGRAD_CTAS, Na // 128)))
     rows = _cdiv(_cdiv(M, splits), 64) * 64
     return _cdiv(M, rows) * Na * ng * r

@@ -5,13 +5,14 @@ and the autograd bridge.  All arithmetic is in libqfx_b200.so.
 Layout conventions (DESIGN.md §3):
   * tokens are stream-major: rows [0, B*T) text (stream index 1), rows [B*T, B*T + B*L) image (stream index 0);
   * frozen weights are plain device tensors in `self.w`, layer-stacked and fused (q|k|v concatenated per stream);
-  * a "site" is one (block, weight group, stream) that may carry LoRA factors, zero-padded to 64 (`A_pad [64*n, in]`,
-    `B_pad [n*out, 64]`, n = 3 for a fused q|k|v site); the trainable nn.Parameters are views into those buffers;
+  * a "site" is one (block, weight group, stream) that may carry LoRA factors, zero-padded to Rp = 64 * ceil(r / 64) (`A_pad [Rp*n, in]`,
+    `B_pad [n*out, Rp]`, n = 3 for a fused q|k|v site); the trainable nn.Parameters are views into those buffers;
   * LoRA gradients accumulate in one flat fp32 buffer `G32` (the all-reduce payload); `G16` holds the bf16 grads.
 """
 from __future__ import annotations
 
 import math
+import numbers
 import os
 import re
 import warnings
@@ -23,7 +24,9 @@ import torch.nn as nn
 from . import lib
 
 BF = torch.bfloat16
-PAD = 64  # LoRA rank is padded to one 64-wide k-block
+PAD = 64  # width of one k-block of the fused GEMM; the LoRA rank is padded to Rp = PAD * ceil(r / PAD) (one or two k-blocks)
+MAX_RANK = 128
+NARROW_RANKS = (64, 32, 16, 8, 4)  # the ranks qfx_lora_wgrad takes (the 64-channel embedder's dA runs in chunks of these widths)
 DEFAULT_TARGETS = ("to_q", "to_k", "to_v", "to_out.0")  # /root/reference/src/qflux/data/config.py:315
 # Device memory left free when the training workspace is planned (the default activation limit is the free device memory minus this):
 # what a step allocates after its workspace.  Measured with tools/recompute_bench.py on an H100 80GB HBM3 (400 W), every Qwen-Image-Edit,
@@ -32,6 +35,28 @@ DEFAULT_TARGETS = ("to_q", "to_k", "to_v", "to_out.0")  # /root/reference/src/qf
 # what that run did not allocate after its workspace: fused-AdamW moments of an optimizer built after the first step and the no-grad
 # workspaces of a validation pass (a few hundred MB each, up to three).
 ACTIVATION_HEADROOM = 4 << 30
+
+
+def padded_rank(r: int) -> int:
+    """Rp: the rank's columns in the padded factor buffers and the T / U workspaces."""
+    return PAD * -(-r // PAD)
+
+
+def check_rank(r) -> None:
+    """The fused path's rank rule: one rank for every adapted module, a multiple of 4 from 4 to MAX_RANK."""
+    if isinstance(r, bool) or not isinstance(r, numbers.Integral) or not (4 <= r <= MAX_RANK and r % 4 == 0):
+        raise NotImplementedError(f"LoRA rank {r!r}: the fused path takes one rank for every adapted module, a multiple of 4 from 4 "
+                                  f"to {MAX_RANK}")
+
+
+def rank_chunks(r: int):
+    """(first rank, width) pieces of [0, r), widths from NARROW_RANKS, largest first: every first rank is a multiple of 8 unless r < 8."""
+    out, c0 = [], 0
+    while c0 < r:
+        w = next(w for w in NARROW_RANKS if w <= r - c0)
+        out.append((c0, w))
+        c0 += w
+    return out
 
 
 class ActivationPlan(NamedTuple):
@@ -74,10 +99,10 @@ class LoraSite:
     """LoRA factors of one (block, group): padded buffers shared by its 1 or 3 member modules (and, for FLUX single
     blocks, by both streams)."""
 
-    def __init__(self, n_slots, d_in, d_out_each, device):
-        self.n = n_slots
-        self.A_pad = torch.zeros(n_slots * PAD, d_in, device=device, dtype=BF)        # rows g*64.. = A of slot g
-        self.B_pad = torch.zeros(n_slots * d_out_each, PAD, device=device, dtype=BF)  # rows g*out.. = B of slot g
+    def __init__(self, n_slots, d_in, d_out_each, rp, device):
+        self.n, self.rp = n_slots, rp
+        self.A_pad = torch.zeros(n_slots * rp, d_in, device=device, dtype=BF)        # rows g*Rp.. = A of slot g
+        self.B_pad = torch.zeros(n_slots * d_out_each, rp, device=device, dtype=BF)  # rows g*out.. = B of slot g
         self.members = {}  # slot -> (name, A_param, B_param, gA_off, gB_off, d_in, d_out)
         self.r = 0
 
@@ -211,7 +236,7 @@ class FusedMMDiTBase(nn.Module):
         self.sites = {}          # (l, grp, s) -> LoraSite   (l = -1: input embedders)
         self.mod_sites = {}      # kind -> dict(idx=[row indices], names=[...], A=[n, r, D], B=[n, C, r], ga, gb)  (AdaLN linears)
         self._lora_params = {}   # PEFT name -> nn.Parameter
-        self.lora_scaling, self.lora_rank = 0.0, 0
+        self.lora_scaling, self.lora_rank, self.lora_rp = 0.0, 0, PAD
         self.adapter_name, self.peft_config = "default", {}
         self.G32 = self.G16 = None
         self._ws = self._ws_key = None
@@ -555,7 +580,9 @@ class FusedMMDiTBase(nn.Module):
                     raise NotImplementedError(f"LoraConfig.{attr}={getattr(cfg, attr)!r}: the fused path implements plain LoRA (dropout 0, no bias)")
             if getattr(cfg, "rank_pattern", None) or getattr(cfg, "alpha_pattern", None):
                 raise NotImplementedError("per-module rank / alpha patterns are not supported by the fused path")
+        check_rank(cfg.r)
         r, lora_alpha = int(cfg.r), float(cfg.lora_alpha)
+        rp = padded_rank(r)
         target_modules = cfg.target_modules
         if isinstance(target_modules, (set, tuple)):
             target_modules = list(target_modules)
@@ -566,8 +593,6 @@ class FusedMMDiTBase(nn.Module):
         self.adapter_name = adapter_name
         self.peft_config = {adapter_name: cfg}
         self._hf_peft_config_loaded = True
-        if r not in (4, 8, 16, 32, 64):
-            raise NotImplementedError(f"LoRA rank {r}: the fused kernels take r in (4, 8, 16, 32, 64)")
         if self._lora_params:
             raise lib.QfxError("an adapter is already attached")
         table = dict(self._linear_table())
@@ -589,18 +614,18 @@ class FusedMMDiTBase(nn.Module):
         wanted_mods = [full for full in mod_table if match(full)]
         if not wanted and not wanted_mods:
             raise lib.QfxError(f"no LoRA-capable module matches target_modules={target_modules!r}")
-        self.lora_rank, self.lora_scaling = r, float(lora_alpha) / r
+        self.lora_rank, self.lora_rp, self.lora_scaling = r, rp, float(lora_alpha) / r
         g = torch.Generator(device=self.dev).manual_seed(seed)
         off = 0
         for full in wanted:
             (l, grp), streams, slot, d_in, d_out, n_slots = table[full]
             site = self.sites.get((l, grp, streams[0]))
             if site is None:
-                site = LoraSite(n_slots, d_in, d_out, self.dev)
+                site = LoraSite(n_slots, d_in, d_out, rp, self.dev)
                 for s in streams:
                     self.sites[(l, grp, s)] = site
             site.r = r
-            A_view = site.A_pad[slot * PAD: slot * PAD + r]            # [r, in]  contiguous
+            A_view = site.A_pad[slot * rp: slot * rp + r]              # [r, in]  contiguous
             B_view = site.B_pad[slot * d_out:(slot + 1) * d_out, :r]   # [out, r] strided view
             if init_lora_weights == "gaussian":
                 A_view.copy_(torch.randn(r, d_in, device=self.dev, generator=g) / r)
@@ -642,7 +667,7 @@ class FusedMMDiTBase(nn.Module):
         self.G16 = torch.zeros(off, device=self.dev, dtype=BF)
         self._gnorm_sq = torch.zeros(1, device=self.dev, dtype=torch.float32)
         self._gnorm_parts = torch.zeros(lib.DET_NORM_PARTIALS, device=self.dev, dtype=torch.float32)  # deterministic finalize
-        self._gscratch = torch.zeros(5 * self.D * PAD, device=self.dev, dtype=torch.float32)
+        self._gscratch = torch.zeros(5 * self.D * rp, device=self.dev, dtype=torch.float32)
         self._ws = self._ws_key = None  # per-block saved tensors depend on which sites exist
         self._train_ws, self._infer_ws = None, {}
         self._infer_graphs.clear()
@@ -962,31 +987,31 @@ class FusedMMDiTBase(nn.Module):
         if site is None:
             return None, None
         Tb = ws["loraT"][(l, grp, s)]
-        lib.gemm([lib.gemm_problem(X, site.A_pad, Tb)], site.n * PAD, X.shape[1], alpha=self.lora_scaling)
+        lib.gemm([lib.gemm_problem(X, site.A_pad, Tb)], site.n * site.rp, X.shape[1], alpha=self.lora_scaling)
         return site, Tb
 
     def _lora_T_pair(self, ws, l, grp, src):
-        """`_lora_T` for the image and the text stream of one weight group in ONE launch (two problems): these [M, 64 g] projections
+        """`_lora_T` for the image and the text stream of one weight group in ONE launch (two problems): these [M, Rp g] projections
         are latency-bound on 8-75 CTAs each, so running them side by side halves their cost.  Returns {s: (site, T)}."""
         res, probs = {}, []
         for s in (0, 1):
             site = self._site(l, grp, s)
             res[s] = (site, None if site is None else ws["loraT"][(l, grp, s)])
             if site is not None:
-                probs.append((site.n, lib.gemm_problem(self._rows(ws, src, s), site.A_pad, res[s][1])))
+                probs.append((site.n * site.rp, lib.gemm_problem(self._rows(ws, src, s), site.A_pad, res[s][1])))
         K = src.shape[1]
         if len(probs) == 2 and probs[0][0] == probs[1][0]:
-            lib.gemm([p for _, p in probs], probs[0][0] * PAD, K, alpha=self.lora_scaling)
+            lib.gemm([p for _, p in probs], probs[0][0], K, alpha=self.lora_scaling)
         else:
             for n, p in probs:
-                lib.gemm([p], n * PAD, K, alpha=self.lora_scaling)
+                lib.gemm([p], n, K, alpha=self.lora_scaling)
         return res
 
     def _embed_fwd(self, ws, key, s, X, dst):
         """Input embedder `key` (x_embedder / context_embedder / img_in / txt_in) with its optional fused LoRA pair."""
         W, b = self._wb(-1, key, s)
         site, Tb = self._lora_T(ws, -1, key, s, X)
-        kw = dict(A2=Tb, B2=site.B_pad, kb2=1) if site is not None else {}
+        kw = dict(A2=Tb, B2=site.B_pad, kb2=site.rp // PAD) if site is not None else {}
         lib.gemm([lib.gemm_problem(X, W, dst, bias=b, **kw)], self.D, X.shape[1])
         ws["embed_in_" + key] = X
 
@@ -1004,7 +1029,7 @@ class FusedMMDiTBase(nn.Module):
             site, Tb = lora[s]
             kw = {}
             if site is not None:
-                kw = dict(A2=Tb, B2=site.B_pad, kb2=1)
+                kw = dict(A2=Tb, B2=site.B_pad, kb2=site.rp // PAD)
             for k, v in epi.items():
                 if v is None:
                     continue
@@ -1027,15 +1052,16 @@ class FusedMMDiTBase(nn.Module):
     def _lora_U_problems(self, ws, l, grp, s, dY, n_out_each):
         """GEMM problems of U_g = scaling * dY_g . B_g for the slots g of one site (U feeds the fused dgrad and dA)."""
         site = self._site(l, grp, s)
-        U = self._rows(ws, ws["U"], s)[:, : site.n * PAD]
+        rp = site.rp
+        U = self._rows(ws, ws["U"], s)[:, : site.n * rp]
         return [lib.gemm_problem(dY[:, g * n_out_each:(g + 1) * n_out_each], site.B_pad[g * n_out_each:(g + 1) * n_out_each],
-                                 U[:, g * PAD:(g + 1) * PAD]) for g in range(site.n)]
+                                 U[:, g * rp:(g + 1) * rp]) for g in range(site.n)]
 
     def _lora_wgrads(self, ws, l, grp, s, dY, Xsaved, n_out_each):
         """Weight gradients of one site on the tensor cores: dB_g[out, r] += dY_g^T T_g (grouped-diagonal), dA_g[r, in] += U_g^T X."""
         site = self._site(l, grp, s)
-        r, Tb = site.r, ws["loraT"][(l, grp, s)]
-        U = self._rows(ws, ws["U"], s)[:, : site.n * PAD]
+        r, rp, Tb = site.r, site.rp, ws["loraT"][(l, grp, s)]
+        U = self._rows(ws, ws["U"], s)[:, : site.n * rp]
         gB, gA = [], []
         for g in range(site.n):
             if g in site.members:
@@ -1050,28 +1076,31 @@ class FusedMMDiTBase(nn.Module):
         wgrad_tc(dY, Tb, gB, r, 1, r, mode=1 if site.n > 1 else 0, Dg=n_out_each if site.n > 1 else 0, **det)
         if Xsaved.shape[1] % 128 == 0:
             wgrad_tc(Xsaved, U, gA, 1, Xsaved.shape[1], r, mode=0, **det)
-        else:  # 64-channel latent embedder: too narrow for the wgmma tile, a [r, 64] result on the CUDA cores
+        else:  # 64-channel latent embedder: too narrow for the wgmma tile, a [r, 64] result on the CUDA cores, in rank chunks of
+            # the widths that kernel takes (disjoint columns of U and rows of dA)
+            d_in = Xsaved.shape[1]
             for g in range(site.n):
-                (lib.lora_wgrad_det if det else lib.lora_wgrad)(Xsaved, U[:, g * PAD:(g + 1) * PAD], gA[g], 1, Xsaved.shape[1], r, **det)
-        return U, site.A_pad, site.n
+                for c0, w in rank_chunks(r):
+                    (lib.lora_wgrad_det if det else lib.lora_wgrad)(Xsaved, U[:, g * rp + c0:(g + 1) * rp], gA[g][c0 * d_in:], 1, d_in, w, **det)
+        return U, site.A_pad, site.n * rp // PAD
 
     def _lora_bwd(self, ws, l, grp, s, dY, Xsaved, n_out_each):
         """LoRA part of a linear's backward for one site: U = s*dY.B (for the fused dgrad) and the weight gradients.
         dY [M_s, n_slots*out]; Xsaved [M_s, in] is the linear's input (for dA)."""
         if self._site(l, grp, s) is None:
             return None
-        lib.gemm(self._lora_U_problems(ws, l, grp, s, dY, n_out_each), PAD, n_out_each, trans_b=True, alpha=self.lora_scaling)
+        lib.gemm(self._lora_U_problems(ws, l, grp, s, dY, n_out_each), self.lora_rp, n_out_each, trans_b=True, alpha=self.lora_scaling)
         return self._lora_wgrads(ws, l, grp, s, dY, Xsaved, n_out_each)
 
     def _lora_bwd_pair(self, ws, l, grp, dY, Xsaved, n_out_each):
         """`_lora_bwd` for both streams of a weight group with ALL their U projections (up to 3 slots x 2 streams) in one launch.
-        dY / Xsaved are stream-major [M, .] buffers.  Returns {s: (U, A_pad, n) | None}."""
+        dY / Xsaved are stream-major [M, .] buffers.  Returns {s: (U, A_pad, kb2 = n Rp / 64) | None}."""
         probs = []
         for s in (0, 1):
             if self._site(l, grp, s) is not None:
                 probs += self._lora_U_problems(ws, l, grp, s, self._rows(ws, dY, s), n_out_each)
         if probs:
-            lib.gemm(probs, PAD, n_out_each, trans_b=True, alpha=self.lora_scaling)
+            lib.gemm(probs, self.lora_rp, n_out_each, trans_b=True, alpha=self.lora_scaling)
         return {s: (self._lora_wgrads(ws, l, grp, s, self._rows(ws, dY, s), self._rows(ws, Xsaved, s), n_out_each)
                     if self._site(l, grp, s) is not None else None) for s in (0, 1)}
 
@@ -1326,7 +1355,8 @@ class FusedMMDiTBase(nn.Module):
             d_in, d_out = site.A_pad.shape[1], site.B_pad.shape[0] // site.n
             for M in (B * Limg, B * T, B * S):
                 n = max(n, lib.det_scratch_wgrad_tc(M, site.n * d_out, 1, site.r))
-                n = max(n, lib.det_scratch_wgrad_tc(M, d_in, site.n, site.r) if d_in % 128 == 0 else lib.det_scratch_wgrad(M, d_in, site.r))
+                n = max(n, lib.det_scratch_wgrad_tc(M, d_in, site.n, site.r) if d_in % 128 == 0 else
+                        max(lib.det_scratch_wgrad(M, d_in, w) for _, w in rank_chunks(site.r)))
         return n
 
     def _fixed_entries(self, B, T, Limg, train, nblk, extra, det=False):
@@ -1338,11 +1368,11 @@ class FusedMMDiTBase(nn.Module):
         pre = [("X", (nblk + 1 if train else 2, M, D), BF), ("xm", (M, D), BF), ("h", (M, 4 * D), BF),
                ("Q", (B, H, S, 128), BF), ("K", (B, H, S, 128), BF), ("V", (B, H, S, 128), BF)]
         post = [("hn", (Mi, D), BF), ("pred", (Mi, self.C_out), BF), ("fstats", (2, Mi), f32)]
-        post += [(("loraT", key), (Mi if key[2] == 0 else B * T, site.n * PAD), BF) for key, site in self.sites.items()]
+        post += [(("loraT", key), (Mi if key[2] == 0 else B * T, site.n * site.rp), BF) for key, site in self.sites.items()]
         if train:
             post += [("dX", (2, M, D), BF), ("dY", (M, D), BF), ("dbig", (M, 4 * D), BF), ("dqkv", (M, 3 * D), BF), ("dxm", (M, D), BF),
                      ("dOj", (B, H, S, 128), BF), ("dK", (B, H, S, 128), BF), ("dV", (B, H, S, 128), BF), ("dQ", (B, H, S, 128), f32),
-                     ("delta", (B, H, S), f32), ("U", (M, 3 * PAD), BF), ("dhn", (Mi, D), BF), ("dpred", (Mi, self.C_out), BF),
+                     ("delta", (B, H, S), f32), ("U", (M, 3 * self.lora_rp), BF), ("dhn", (Mi, D), BF), ("dpred", (Mi, self.C_out), BF),
                      ("loss", (1,), f32)]
             if det:
                 post.append(("det_scratch", (self._det_scratch_floats(B, T, Limg),), f32))
