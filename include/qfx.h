@@ -329,6 +329,53 @@ int qfx_fused_adam8bit(const qfx_adamw_tensor* tensors, const int* chunks, int n
                        int min_8bit_size, void* stream);
 
 /* ------------------------------------------------------------------------------------------------------------------
+ * Sharded optimizer state (qflux_b200/optim.py shard_state=True; replaces, per data-parallel rank, optimizer.step() of
+ * base_trainer.py:528-533).  A rank owns the contiguous range [state_base, state_base + n_state) of the flat gradient: whole chunks of
+ * the tables above (`chunks` / n_chunks is the rank's sub-list; n_chunks == 0 launches nothing).  Its state arrays hold that range
+ * only, element fi at index fi - state_base; every chunk's gradient range must lie inside it.  `sumsq` is given, not computed: the
+ * caller sums ||grad * pre_scale||^2 over the ranks' slices.  Per element each computes what its replicated form computes with that
+ * sumsq; the replicated kernels run unchanged.  No host synchronisation; the same inputs give the same bits.
+ *
+ * qfx_sumsq_det: out[0] = ||x * pre_scale||^2 over n >= 0 floats, QFX_DET_NORM_PARTIALS grid-stride partials in scratch
+ *   (scratch_floats >= QFX_DET_NORM_PARTIALS) added in a fixed order.  Two launches.
+ * qfx_fused_adamw_slice: qfx_fused_adamw / _det on the slice.  One launch.
+ * qfx_fused_adam8bit_slice: qfx_fused_adam8bit on the slice.  state1 / state2 are n_state bytes; state_offsets is the slice's own
+ *   table (tensor i's absmax / fp32 states at state_offsets[i] + e / QFX_ADAM8BIT_BLOCK / + e in the slice's absmax* / s*_32 arrays,
+ *   e the element of the tensor; entries may be negative).  One launch.
+ * qfx_prodigy_slice_partials: pass A of qfx_fused_prodigy on the slice.  The chunks are entries [chunk0, chunk0 + n_chunks) of the
+ *   full table of n_parts chunks; their (sum g (p0 - p), sum |s|) go to part[2 (chunk0 + i)], part[2 (chunk0 + i) + 1] (fp64).
+ *   One launch.
+ * qfx_prodigy_slice_update: once `part` holds all n_parts chunks' partials (the ranks' slices gathered), the scalar update of
+ *   qfx_fused_prodigy over them in chunk order (the same bits as the replicated optimizer from the same partials), then pass B on
+ *   the slice.  Two launches (one when n_chunks == 0). */
+int qfx_sumsq_det(const float* x, int64_t n, float pre_scale, float* out, float* scratch, int64_t scratch_floats, void* stream);
+int qfx_fused_adamw_slice(const qfx_adamw_tensor* tensors, const int* chunks, int n_chunks, const float* grad, int64_t n_grad,
+                          int64_t state_base, int64_t n_state, float* exp_avg, float* exp_avg_sq, const float* sumsq, float pre_scale,
+                          float max_norm, float lr, float beta1, float beta2, float eps, float weight_decay, int step, void* stream);
+int qfx_fused_adam8bit_slice(const qfx_adamw_tensor* tensors, const int* chunks, int n_chunks, const int64_t* state_offsets,
+                             const float* grad, int64_t n_grad, int64_t state_base, int64_t n_state, unsigned char* state1,
+                             unsigned char* state2, float* absmax1, float* absmax2, float* s1_32, float* s2_32, const float* qmap1,
+                             const float* qmap2, const float* sumsq, float pre_scale, float max_norm, float lr, float beta1, float beta2,
+                             float eps, float weight_decay, int step, int min_8bit_size, void* stream);
+int qfx_prodigy_slice_partials(const qfx_adamw_tensor* tensors, const int* chunks, int n_chunks, int chunk0, const float* grad,
+                               int64_t n_grad, int64_t state_base, int64_t n_state, float* exp_avg, float* exp_avg_sq, float* s,
+                               const void* p0, const double* scalars, const float* sumsq, double* part, int n_parts, float pre_scale,
+                               float max_norm, double lr, double beta1, double beta2, double beta3, double weight_decay, int decouple,
+                               int use_bias_correction, int safeguard_warmup, double d0, void* stream);
+int qfx_prodigy_slice_update(const qfx_adamw_tensor* tensors, const int* chunks, int n_chunks, int64_t n_grad, int64_t state_base,
+                             int64_t n_state, const float* exp_avg, const float* exp_avg_sq, double* scalars, const double* part,
+                             int n_parts, double lr, double beta1, double beta2, double beta3, double eps, double weight_decay,
+                             int decouple, int use_bias_correction, double d0, double d_coef, double growth_rate, void* stream);
+/* qfx_lora_pack / qfx_lora_unpack: the weight all-gather's staging.  For every element of the listed chunks whose gradient offset fi
+ * lies in [g_lo, g_hi):  flat[fi - g_lo] = param element (pack),  param element = flat[fi - g_lo] (unpack);  flat is bf16, 2-byte
+ * aligned; nothing else is read or written.  Runs of 8 elements within one row move as 16-byte vectors where both sides are 16-byte
+ * aligned.  No atomics; one launch (none when n_chunks == 0 or g_hi == g_lo). */
+int qfx_lora_pack(const qfx_adamw_tensor* tensors, const int* chunks, int n_chunks, int64_t g_lo, int64_t g_hi, void* flat,
+                  void* stream);
+int qfx_lora_unpack(const qfx_adamw_tensor* tensors, const int* chunks, int n_chunks, int64_t g_lo, int64_t g_hi, const void* flat,
+                    void* stream);
+
+/* ------------------------------------------------------------------------------------------------------------------
  * NF4 frozen weights (4-bit base checkpoints: bitsandbytes `Linear4bit`, whose forward dequantizes the weight to bf16 and runs a
  * plain matmul, bitsandbytes/functional.py dequantize_4bit).  One launch dequantizes up to QFX_NF4_MAX_SEGMENTS tensors (the NF4
  * matrices of one block) into bf16:  out[i] = bf16_rn(NF4[nibble_i] * absmax[i / blocksize])  with the product in fp32,

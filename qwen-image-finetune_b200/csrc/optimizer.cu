@@ -405,3 +405,167 @@ extern "C" int qfx_fused_adamw_det(const qfx_adamw_tensor* tensors_dev, const in
   QFX_CUDA(cudaGetLastError());
   return 0;
 }
+
+/* ---- Sharded optimizer state (qfx.h "slice forms"; qflux_b200/optim.py shard_state=True).  Each data-parallel rank steps only the
+ * chunks of its slice [state_base, state_base + n_state) of the flat gradient and keeps state for that range alone.  The kernels above
+ * index the state by the gradient offset fi; the slice entry points hand them state pointers moved back by state_base, so element fi
+ * lands at state[fi - state_base] and the replicated launches keep their code.  The norm behind the clip is the caller's: sumsq holds
+ * ||grad * pre_scale||^2 summed over the ranks' slices.  Each replaces, for its slice, the reference's optimizer.step()
+ * (/root/reference/src/qflux/trainer/base_trainer.py:528-533). */
+template <typename T>
+static T* state_at(T* p, int64_t state_base) {  // p - state_base, formed on the integer so no pointer leaves the allocation in C++ terms
+  return reinterpret_cast<T*>(reinterpret_cast<uintptr_t>(p) - (uintptr_t)state_base * sizeof(T));
+}
+
+static bool slice_args_ok(int n_chunks, int64_t n_grad, int64_t state_base, int64_t n_state) {
+  return n_chunks >= 0 && n_grad > 0 && state_base >= 0 && n_state >= 0 && state_base + n_state <= n_grad;
+}
+
+extern "C" int qfx_sumsq_det(const float* x, int64_t n, float pre_scale, float* out, float* scratch, int64_t scratch_floats,
+                             void* stream) {
+  QFX_CHECK_ARG(out && n >= 0 && (x || n == 0), "qfx_sumsq_det: bad arguments");
+  QFX_CHECK_ARG(scratch && scratch_floats >= QFX_DET_NORM_PARTIALS, "qfx_sumsq_det: scratch holds %lld floats, needs %d",
+                (long long)scratch_floats, QFX_DET_NORM_PARTIALS);
+  cudaStream_t st = (cudaStream_t)stream;
+  adamw_sumsq_kernel<true><<<QFX_DET_NORM_PARTIALS, 256, 0, st>>>(x, n, pre_scale, scratch);
+  QFX_CUDA(cudaGetLastError());
+  SplitSum S;
+  memset(&S, 0, sizeof(S));
+  S.part = scratch; S.split_stride = 1; S.splits = QFX_DET_NORM_PARTIALS; S.rows = S.cols = 1;
+  S.dst[0] = out; S.rows_per_dst = S.cols_per_dst = 1; S.accumulate = 0;
+  return launch_split_sum(S, st);
+}
+
+extern "C" int qfx_fused_adamw_slice(const qfx_adamw_tensor* tensors_dev, const int* chunks_dev, int n_chunks, const float* grad,
+                                     int64_t n_grad, int64_t state_base, int64_t n_state, float* exp_avg, float* exp_avg_sq,
+                                     const float* sumsq, float pre_scale, float max_norm, float lr, float beta1, float beta2, float eps,
+                                     float weight_decay, int step, void* stream) {
+  QFX_CHECK_ARG(slice_args_ok(n_chunks, n_grad, state_base, n_state) && grad && sumsq && step >= 1 &&
+                    (n_chunks == 0 || (tensors_dev && chunks_dev && exp_avg && exp_avg_sq)),
+                "qfx_fused_adamw_slice: bad arguments");
+  if (n_chunks == 0) return 0;
+  const float bc1 = 1.f - powf(beta1, (float)step), bc2 = 1.f - powf(beta2, (float)step);
+  fused_adamw_kernel<<<n_chunks, 256, 0, (cudaStream_t)stream>>>(tensors_dev, reinterpret_cast<const int2*>(chunks_dev), grad,
+                                                                 state_at(exp_avg, state_base), state_at(exp_avg_sq, state_base), sumsq,
+                                                                 pre_scale, max_norm, lr, beta1, beta2, eps, weight_decay, bc1, sqrtf(bc2));
+  QFX_CUDA(cudaGetLastError());
+  return 0;
+}
+
+extern "C" int qfx_fused_adam8bit_slice(const qfx_adamw_tensor* tensors_dev, const int* chunks_dev, int n_chunks,
+                                        const int64_t* state_offsets, const float* grad, int64_t n_grad, int64_t state_base,
+                                        int64_t n_state, unsigned char* state1, unsigned char* state2, float* absmax1, float* absmax2,
+                                        float* s1_32, float* s2_32, const float* qmap1, const float* qmap2, const float* sumsq,
+                                        float pre_scale, float max_norm, float lr, float beta1, float beta2, float eps, float weight_decay,
+                                        int step, int min_8bit_size, void* stream) {
+  QFX_CHECK_ARG(slice_args_ok(n_chunks, n_grad, state_base, n_state) && grad && sumsq && step >= 1 && min_8bit_size >= 0 &&
+                    (n_chunks == 0 || (tensors_dev && chunks_dev && state_offsets && state1 && state2 && absmax1 && absmax2 && s1_32 &&
+                                       s2_32 && qmap1 && qmap2)),
+                "qfx_fused_adam8bit_slice: bad arguments");
+  QFX_CHECK_ARG(lr >= 0.f, "qfx_fused_adam8bit_slice: needs lr >= 0, got %g", (double)lr);
+  if (n_chunks == 0) return 0;
+  const float c1 = 1.f - powf(beta1, (float)step), c2 = sqrtf(1.f - powf(beta2, (float)step));
+  const float step_size = -lr * c2 / c1, decay = weight_decay > 0.f ? 1.f - lr * weight_decay : 1.f;
+  fused_adam8bit_kernel<<<n_chunks, 256, 0, (cudaStream_t)stream>>>(
+      tensors_dev, reinterpret_cast<const int2*>(chunks_dev), state_offsets, grad, state_at(state1, state_base),
+      state_at(state2, state_base), absmax1, absmax2, s1_32, s2_32, qmap1, qmap2, sumsq, pre_scale, max_norm, beta1, beta2, c2 * eps,
+      step_size, decay, min_8bit_size);
+  QFX_CUDA(cudaGetLastError());
+  return 0;
+}
+
+extern "C" int qfx_prodigy_slice_partials(const qfx_adamw_tensor* tensors_dev, const int* chunks_dev, int n_chunks, int chunk0,
+                                          const float* grad, int64_t n_grad, int64_t state_base, int64_t n_state, float* exp_avg,
+                                          float* exp_avg_sq, float* s, const void* p0, const double* scalars, const float* sumsq,
+                                          double* part, int n_parts, float pre_scale, float max_norm, double lr, double beta1,
+                                          double beta2, double beta3, double weight_decay, int decouple, int use_bias_correction,
+                                          int safeguard_warmup, double d0, void* stream) {
+  QFX_CHECK_ARG(slice_args_ok(n_chunks, n_grad, state_base, n_state) && grad && scalars && sumsq && part && chunk0 >= 0 &&
+                    (int64_t)chunk0 + n_chunks <= n_parts &&
+                    (n_chunks == 0 || (tensors_dev && chunks_dev && exp_avg && exp_avg_sq && s && p0)),
+                "qfx_prodigy_slice_partials: bad arguments");
+  QFX_CHECK_ARG(lr > 0.0 && d0 > 0.0, "qfx_prodigy_slice_partials: needs lr > 0 and d0 > 0");
+  if (n_chunks == 0) return 0;
+  prodigy_pass_a_kernel<<<n_chunks, 256, 0, (cudaStream_t)stream>>>(
+      tensors_dev, reinterpret_cast<const int2*>(chunks_dev), grad, state_at(exp_avg, state_base), state_at(exp_avg_sq, state_base),
+      state_at(s, state_base), state_at(reinterpret_cast<const bf16*>(p0), state_base), scalars, sumsq, pre_scale, max_norm, lr, beta1,
+      beta2, beta3, (float)weight_decay, decouple, use_bias_correction, safeguard_warmup, d0, part + 2 * (int64_t)chunk0);
+  QFX_CUDA(cudaGetLastError());
+  return 0;
+}
+
+extern "C" int qfx_prodigy_slice_update(const qfx_adamw_tensor* tensors_dev, const int* chunks_dev, int n_chunks, int64_t n_grad,
+                                        int64_t state_base, int64_t n_state, const float* exp_avg, const float* exp_avg_sq,
+                                        double* scalars, const double* part, int n_parts, double lr, double beta1, double beta2,
+                                        double beta3, double eps, double weight_decay, int decouple, int use_bias_correction, double d0,
+                                        double d_coef, double growth_rate, void* stream) {
+  QFX_CHECK_ARG(slice_args_ok(n_chunks, n_grad, state_base, n_state) && scalars && part && n_parts > 0 && n_chunks <= n_parts &&
+                    (n_chunks == 0 || (tensors_dev && chunks_dev && exp_avg && exp_avg_sq)),
+                "qfx_prodigy_slice_update: bad arguments");
+  QFX_CHECK_ARG(lr > 0.0 && d0 > 0.0, "qfx_prodigy_slice_update: needs lr > 0 and d0 > 0");
+  cudaStream_t st = (cudaStream_t)stream;
+  prodigy_scalar_kernel<<<1, 256, 0, st>>>(scalars, part, n_parts, lr, beta1, beta2, beta3, use_bias_correction, d0, d_coef, growth_rate);
+  QFX_CUDA(cudaGetLastError());
+  if (n_chunks == 0) return 0;
+  prodigy_pass_b_kernel<<<n_chunks, 256, 0, st>>>(tensors_dev, reinterpret_cast<const int2*>(chunks_dev), state_at(exp_avg, state_base),
+                                                  state_at(exp_avg_sq, state_base), scalars, (float)eps, (float)weight_decay, decouple,
+                                                  beta1 > 0.0);
+  QFX_CUDA(cudaGetLastError());
+  return 0;
+}
+
+namespace qfx {
+// One CTA per chunk: the chunk's elements whose gradient offset lies in [g_lo, g_hi) move between the bf16 parameter (row-strided) and
+// flat[fi - g_lo].  Runs of 8 elements move as one 16-byte vector when a run is one row and both sides are 16-byte aligned.
+template <bool kUnpack>
+__global__ void __launch_bounds__(256) lora_pack_kernel(const qfx_adamw_tensor* __restrict__ tensors, const int2* __restrict__ chunks,
+                                                        int64_t g_lo, int64_t g_hi, bf16* __restrict__ flat) {
+  const int2 ck = chunks[blockIdx.x];
+  const qfx_adamw_tensor t = tensors[ck.x];
+  const int e0 = (int)max((int64_t)ck.y, g_lo - t.grad_offset);
+  const int e1 = (int)min((int64_t)min(t.numel, ck.y + QFX_ADAMW_CHUNK), g_hi - t.grad_offset);
+  if (e0 >= e1) return;
+  bf16* p = reinterpret_cast<bf16*>(t.param);
+  const int64_t fo = t.grad_offset - g_lo;  // flat index of the tensor's element e is fo + e
+  const bool vec = (t.cols & 7) == 0 && (t.ld & 7) == 0 && ((uintptr_t)p & 15) == 0 && (((uintptr_t)flat + 2 * fo) & 15) == 0;
+  const int v0 = vec ? min(e1, (e0 + 7) & ~7) : e1, v1 = vec ? max(v0, e1 & ~7) : e1;  // [v0, v1): whole 8-runs
+  for (int e = v0 + 8 * threadIdx.x; e < v1; e += 8 * blockDim.x) {
+    const int row = e / t.cols, col = e - row * t.cols;
+    uint4* pp = reinterpret_cast<uint4*>(p + (int64_t)row * t.ld + col);
+    uint4* fp = reinterpret_cast<uint4*>(flat + fo + e);
+    if constexpr (kUnpack) *pp = *fp;
+    else *fp = *pp;
+  }
+  const int head = v0 - e0;  // [e0, v0) and [v1, e1): fewer than 8 elements each when vec, everything otherwise
+  for (int i = threadIdx.x; i < head + (e1 - v1); i += blockDim.x) {
+    const int e = i < head ? e0 + i : v1 + (i - head);
+    const int row = e / t.cols, col = e - row * t.cols;
+    bf16* pp = p + (int64_t)row * t.ld + col;
+    if constexpr (kUnpack) *pp = flat[fo + e];
+    else flat[fo + e] = *pp;
+  }
+}
+}  // namespace qfx
+
+template <bool kUnpack>
+static int lora_pack(const char* what, const qfx_adamw_tensor* tensors_dev, const int* chunks_dev, int n_chunks, int64_t g_lo,
+                     int64_t g_hi, void* flat, void* stream) {
+  QFX_CHECK_ARG(n_chunks >= 0 && g_lo >= 0 && g_hi >= g_lo && (n_chunks == 0 || (tensors_dev && chunks_dev && flat)),
+                "%s: bad arguments", what);
+  QFX_CHECK_ARG(((uintptr_t)flat & 1) == 0, "%s: flat must be 2-byte aligned", what);
+  if (n_chunks == 0 || g_hi == g_lo) return 0;
+  lora_pack_kernel<kUnpack><<<n_chunks, 256, 0, (cudaStream_t)stream>>>(tensors_dev, reinterpret_cast<const int2*>(chunks_dev), g_lo, g_hi,
+                                                                         reinterpret_cast<bf16*>(flat));
+  QFX_CUDA(cudaGetLastError());
+  return 0;
+}
+
+extern "C" int qfx_lora_pack(const qfx_adamw_tensor* tensors_dev, const int* chunks_dev, int n_chunks, int64_t g_lo, int64_t g_hi,
+                             void* flat, void* stream) {
+  return lora_pack<false>("qfx_lora_pack", tensors_dev, chunks_dev, n_chunks, g_lo, g_hi, flat, stream);
+}
+
+extern "C" int qfx_lora_unpack(const qfx_adamw_tensor* tensors_dev, const int* chunks_dev, int n_chunks, int64_t g_lo, int64_t g_hi,
+                               const void* flat, void* stream) {
+  return lora_pack<true>("qfx_lora_unpack", tensors_dev, chunks_dev, n_chunks, g_lo, g_hi, const_cast<void*>(flat), stream);
+}

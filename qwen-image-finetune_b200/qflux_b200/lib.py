@@ -461,6 +461,103 @@ def fused_adam8bit(tables, state_offsets, grad, state1, state2, absmax1, absmax2
                     int(min_8bit_size), cur_stream()), "qfx_fused_adam8bit")
 
 
+# Sharded optimizer state (qfx.h "slice forms"; optim.py shard_state=True).  `chunk_range` = (c0, c1) selects entries [c0, c1) of the
+# tables' chunk list (sharding.SlicePlan); the state arrays hold the flat-gradient range starting at `state_base`.
+_sumsq_det = _sig("qfx_sumsq_det", _vp, _i64, _f, _vp, _vp, _i64, _vp)
+_adamw_slice = _sig("qfx_fused_adamw_slice", _vp, _vp, _i, _vp, _i64, _i64, _i64, _vp, _vp, _vp, _f, _f, _f, _f, _f, _f, _f, _i, _vp)
+_adam8bit_slice = _sig("qfx_fused_adam8bit_slice", _vp, _vp, _i, _vp, _vp, _i64, _i64, _i64, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp,
+                       _f, _f, _f, _f, _f, _f, _f, _i, _i, _vp)
+_prodigy_a = _sig("qfx_prodigy_slice_partials", _vp, _vp, _i, _i, _vp, _i64, _i64, _i64, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i, _f, _f,
+                  _d, _d, _d, _d, _d, _i, _i, _i, _d, _vp)
+_prodigy_b = _sig("qfx_prodigy_slice_update", _vp, _vp, _i, _i64, _i64, _i64, _vp, _vp, _vp, _vp, _i, _d, _d, _d, _d, _d, _d, _i, _i, _d,
+                  _d, _d, _vp)
+_pack = _sig("qfx_lora_pack", _vp, _vp, _i, _i64, _i64, _vp, _vp)
+_unpack = _sig("qfx_lora_unpack", _vp, _vp, _i, _i64, _i64, _vp, _vp)
+_KERNELS_PER_CALL.update({"qfx_sumsq_det": 2, "qfx_prodigy_slice_update": 2})
+
+
+def _sub_chunks(tables, chunk_range):
+    """(tensor table pointer, pointer to chunk c0, number of chunks) of a chunk range."""
+    raw, chunks = tables
+    c0, c1 = chunk_range
+    assert 0 <= c0 <= c1 <= chunks.shape[0]
+    return ptr(raw), C.c_void_p(chunks.data_ptr() + 8 * c0), c1 - c0
+
+
+def sumsq_det(x, pre_scale, out, *, scratch):
+    """out[0] = ||x * pre_scale||^2 (fp32, x contiguous, any length), summed in a fixed order."""
+    require_cuda(x, out, scratch)
+    assert x.dtype == torch.float32 and x.is_contiguous()
+    check(_sumsq_det(ptr(x), x.numel(), float(pre_scale), ptr(out), *_scratch(scratch), cur_stream()), "qfx_sumsq_det")
+
+
+def _state(t, n):
+    assert t.is_contiguous() and t.numel() >= n
+    return ptr(t)
+
+
+def fused_adamw_slice(tables, chunk_range, state_base, grad, exp_avg, exp_avg_sq, sumsq, pre_scale, max_norm, lr, beta1, beta2, eps,
+                      weight_decay, step):
+    """fused_adamw on the chunks of `chunk_range`, with moments of the slice only and the clip from the given sumsq."""
+    require_cuda(grad, exp_avg, exp_avg_sq, sumsq)
+    n = exp_avg.numel()
+    check(_adamw_slice(*_sub_chunks(tables, chunk_range), ptr(grad), grad.numel(), int(state_base), n, _state(exp_avg, n),
+                       _state(exp_avg_sq, n), ptr(sumsq), float(pre_scale), float(max_norm), float(lr), float(beta1), float(beta2),
+                       float(eps), float(weight_decay), int(step), cur_stream()), "qfx_fused_adamw_slice")
+
+
+def fused_adam8bit_slice(tables, chunk_range, state_base, state_offsets, grad, state1, state2, absmax1, absmax2, s1_32, s2_32, qmap1,
+                         qmap2, sumsq, pre_scale, max_norm, lr, beta1, beta2, eps, weight_decay, step, min_8bit_size):
+    """fused_adam8bit on the chunks of `chunk_range`: codes of the slice, the slice's absmax / fp32 states at its own `state_offsets`."""
+    require_cuda(state_offsets, grad, state1, state2, absmax1, absmax2, s1_32, s2_32, qmap1, qmap2, sumsq)
+    assert state1.dtype == state2.dtype == torch.uint8 and state_offsets.dtype == torch.int64 and qmap1.numel() == qmap2.numel() == 256
+    n = state1.numel()
+    check(_adam8bit_slice(*_sub_chunks(tables, chunk_range), ptr(state_offsets), ptr(grad), grad.numel(), int(state_base), n,
+                          _state(state1, n), _state(state2, n), ptr(absmax1), ptr(absmax2), ptr(s1_32), ptr(s2_32), ptr(qmap1), ptr(qmap2),
+                          ptr(sumsq), float(pre_scale), float(max_norm), float(lr), float(beta1), float(beta2), float(eps),
+                          float(weight_decay), int(step), int(min_8bit_size), cur_stream()), "qfx_fused_adam8bit_slice")
+
+
+def prodigy_slice_partials(tables, chunk_range, state_base, grad, exp_avg, exp_avg_sq, s, p0, scalars, sumsq, part, pre_scale, max_norm,
+                           lr, beta1, beta2, beta3, weight_decay, decouple, use_bias_correction, safeguard_warmup, d0):
+    """Pass A of fused_prodigy on the slice; its chunks' fp64 partials go to part[2 c], part[2 c + 1] (c = the chunk's index in the
+    full table; part holds 2 x every chunk)."""
+    require_cuda(grad, exp_avg, exp_avg_sq, s, p0, scalars, sumsq, part)
+    assert p0.dtype == torch.bfloat16 and scalars.dtype == part.dtype == torch.float64 and part.is_contiguous()
+    n = exp_avg.numel()
+    check(_prodigy_a(*_sub_chunks(tables, chunk_range), int(chunk_range[0]), ptr(grad), grad.numel(), int(state_base), n,
+                     _state(exp_avg, n), _state(exp_avg_sq, n), _state(s, n), _state(p0, n), ptr(scalars), ptr(sumsq), ptr(part),
+                     part.numel() // 2, float(pre_scale), float(max_norm), float(lr), float(beta1), float(beta2), float(beta3),
+                     float(weight_decay), int(bool(decouple)), int(bool(use_bias_correction)), int(bool(safeguard_warmup)), float(d0),
+                     cur_stream()), "qfx_prodigy_slice_partials")
+
+
+def prodigy_slice_update(tables, chunk_range, state_base, n_grad, exp_avg, exp_avg_sq, scalars, part, lr, beta1, beta2, beta3, eps,
+                         weight_decay, decouple, use_bias_correction, d0, d_coef, growth_rate):
+    """The scalar update of fused_prodigy from every chunk's partials in `part`, then pass B on the slice."""
+    require_cuda(exp_avg, exp_avg_sq, scalars, part)
+    assert scalars.dtype == part.dtype == torch.float64 and scalars.numel() == PRODIGY_SCALARS
+    n = exp_avg.numel()
+    check(_prodigy_b(*_sub_chunks(tables, chunk_range), int(n_grad), int(state_base), n, _state(exp_avg, n), _state(exp_avg_sq, n),
+                     ptr(scalars), ptr(part), part.numel() // 2, float(lr), float(beta1), float(beta2), float(beta3), float(eps),
+                     float(weight_decay), int(bool(decouple)), int(bool(use_bias_correction)), float(d0), float(d_coef), float(growth_rate),
+                     cur_stream()), "qfx_prodigy_slice_update")
+
+
+def lora_pack(tables, chunk_range, g_lo, g_hi, flat):
+    """flat[fi - g_lo] = the LoRA weight at flat-gradient offset fi, for fi in [g_lo, g_hi) within the chunks of `chunk_range`."""
+    require_cuda(flat)
+    assert flat.dtype == torch.bfloat16 and flat.is_contiguous() and flat.numel() >= g_hi - g_lo
+    check(_pack(*_sub_chunks(tables, chunk_range), int(g_lo), int(g_hi), ptr(flat), cur_stream()), "qfx_lora_pack")
+
+
+def lora_unpack(tables, chunk_range, g_lo, g_hi, flat):
+    """The inverse of lora_pack: the LoRA weights at offsets [g_lo, g_hi) within the chunks of `chunk_range` = flat[fi - g_lo]."""
+    require_cuda(flat)
+    assert flat.dtype == torch.bfloat16 and flat.is_contiguous() and flat.numel() >= g_hi - g_lo
+    check(_unpack(*_sub_chunks(tables, chunk_range), int(g_lo), int(g_hi), ptr(flat), cur_stream()), "qfx_lora_unpack")
+
+
 def lora_wgrad(P, Q, G, gs_i, gs_j, r):
     """G[i*gs_i + j*gs_j] += sum_m P[m,i] Q[m,j], j < r.  G fp32."""
     require_cuda(P, Q, G)

@@ -23,6 +23,8 @@ The same two-slot ring (`BlockRing`) has two more fill sources: `Nf4Blocks` dequ
 """
 from __future__ import annotations
 
+import bisect
+import contextlib
 import os
 
 import torch
@@ -283,30 +285,47 @@ class GradExchange:
         for evs in self._peer_events:
             s.wait_event(evs[k])
 
+    def _reduce_slice(self, bounds):
+        """Phase 1 with slice q = bounds[q]: this rank's slice of G32 <- the rank-ordered sum of every rank's slice.  Returns the
+        gathered copies of every rank's G32 on CPU models (phase 2 reuses them)."""
+        from . import lib
+        g32 = self.model.G32
+        lo, hi = bounds[self.rank]
+        if not self.cuda:
+            bufs = [torch.empty_like(g32) for _ in range(self.world)]
+            dist.all_gather(bufs, g32, group=self.host)
+            if hi > lo:
+                lib.dp_reduce_det([b[lo:hi] for b in bufs], g32[lo:hi])
+            return bufs
+        if g32.data_ptr() != self._buf.ptr:
+            raise RuntimeError("GradExchange: the model's G32 was replaced after the exchange was set up (add_adapter during "
+                               "data-parallel training); call model.close() on every rank first")
+        self._point(0)
+        if hi > lo:
+            lib.dp_reduce_det([p + lo * 4 for p in self._ptrs], g32[lo:hi])
+        self._point(1)
+        return None
+
+    def reduce_scatter(self, bounds):
+        """Slice bounds[rank] of G32 <- the rank-ordered sum of every rank's G32 there; the rest of G32 is left as it is (collective;
+        asynchronous on the current stream).  The sharded optimizer's exchange: phase 1 without the all-gather.  The point after the
+        reduce also orders the next write of G32 after every peer's reads of it."""
+        with torch.cuda.device(self.dev) if self.cuda else contextlib.nullcontext():
+            self._reduce_slice(bounds)
+
     def all_reduce(self):
         """G32 <- the rank-ordered sum of every rank's G32 (collective; asynchronous on the current stream)."""
         from . import lib
         g32 = self.model.G32
         if not self.cuda:
-            bufs = [torch.empty_like(g32) for _ in range(self.world)]
-            dist.all_gather(bufs, g32, group=self.host)
-            lo, hi = self.bounds[self.rank]
-            if hi > lo:
-                lib.dp_reduce_det([b[lo:hi] for b in bufs], g32[lo:hi])
+            bufs = self._reduce_slice(self.bounds)
             dist.all_gather(bufs, g32, group=self.host)
             for r, (lo, hi) in enumerate(self.bounds):
                 if r != self.rank:
                     g32[lo:hi] = bufs[r][lo:hi]
             return
-        if g32.data_ptr() != self._buf.ptr:
-            raise RuntimeError("GradExchange: the model's G32 was replaced after the exchange was set up (add_adapter during "
-                               "data-parallel training); call model.close() on every rank first")
         with torch.cuda.device(self.dev):
-            self._point(0)
-            lo, hi = self.bounds[self.rank]
-            if hi > lo:
-                lib.dp_reduce_det([p + lo * 4 for p in self._ptrs], g32[lo:hi])
-            self._point(1)
+            self._reduce_slice(self.bounds)
             for i in range(1, self.world):
                 r = (self.rank + i) % self.world
                 lo, hi = self.bounds[r]
@@ -365,3 +384,178 @@ class Fp8Blocks(BlockRing):
         from . import lib
         lib.fp8_expand([(c[l].reshape(-1), self.gbuf[s, self.rings[k].offset: self.rings[k].offset + self.rings[k].numel])
                         for k, c in self.stacks.items()])
+
+
+class SlicePlan:
+    """Which part of the flat LoRA gradient each data-parallel rank's sharded optimizer owns (optim.py shard_state=True).
+
+    The members (the optimizer's (LoRA tensor, gradient offset) pairs) are taken in gradient-offset order, `members`, and tiled into
+    chunks of <= lib.ADAMW_CHUNK consecutive elements of one tensor, `chunks`, as lib.adamw_tables tiles them; a sharded optimizer
+    builds its tables from `members`.  The chunk list is split into `world` contiguous ranges balanced by element count: cut q sits at
+    the chunk boundary nearest to q / world of the elements, so every slice is within one chunk of the mean.  Cuts fall on chunk
+    boundaries only, so an 8-bit Adam block (256 elements, which divides the chunk) is never cut and every per-chunk Prodigy partial
+    belongs to one rank.  Slice q's gradient range `bounds[q]` runs from its first chunk's offset to the next slice's (0 and
+    G32.numel() at the ends): the slices partition G32, which keeps its layout.  `order[j]` is the index in the caller's member list
+    of `members[j]`, and `table_chunk[c]` the index of chunk c in the chunk list of the caller's order (the replicated optimizer's
+    tables).  The exchange, the optimizer's state, its state_dict and the tests all read their slice bounds from here."""
+
+    def __init__(self, members, n_grad: int, world: int):
+        from . import lib
+        members = list(members)
+        self.world, self.n_grad = int(world), int(n_grad)
+        self.order = sorted(range(len(members)), key=lambda i: members[i][1])
+        self.members = [members[i] for i in self.order]
+        first, c = [], 0  # first chunk of each member in the caller's order
+        for p, _ in members:
+            first.append(c)
+            c += -(-p.numel() // lib.ADAMW_CHUNK)
+        chunks, table_chunk, end = [], [], 0  # (member, first element, gradient offset, elements)
+        for j, (p, off) in enumerate(self.members):
+            n = p.numel()
+            if off < end or off + n > n_grad:
+                raise ValueError("SlicePlan: members must sit in disjoint ranges of the flat gradient")
+            chunks += [(j, e, off + e, min(lib.ADAMW_CHUNK, n - e)) for e in range(0, n, lib.ADAMW_CHUNK)]
+            table_chunk += [first[self.order[j]] + k for k in range(-(-n // lib.ADAMW_CHUNK))]
+            end = off + n
+        self.chunks, self.table_chunk = chunks, table_chunk
+        prefix = [0]
+        for c in chunks:
+            prefix.append(prefix[-1] + c[3])
+        total, cuts = prefix[-1], [0]
+        for q in range(1, world):
+            target = total * q / world
+            k = bisect.bisect_left(prefix, target, lo=cuts[-1])
+            if k > cuts[-1] and (k == len(prefix) or target - prefix[k - 1] <= prefix[k] - target):
+                k -= 1
+            cuts.append(min(k, len(chunks)))
+        cuts.append(len(chunks))
+        self.chunk_ranges = [(cuts[q], cuts[q + 1]) for q in range(world)]
+        start = [c[2] for c in chunks] + [self.n_grad]
+        start[0] = 0
+        self.bounds = [(start[c0], start[c1]) for c0, c1 in self.chunk_ranges]
+        self._starts = [c[2] for c in chunks]
+        self.elements = [prefix[c1] - prefix[c0] for c0, c1 in self.chunk_ranges]
+
+    def pieces(self, q):
+        """(index into `members`, first element, end element) of every tensor part in slice q, in gradient order."""
+        out = []
+        for i, e, _, n in self.chunks[slice(*self.chunk_ranges[q])]:
+            if out and out[-1][0] == i and out[-1][2] == e:
+                out[-1] = (i, out[-1][1], e + n)
+            else:
+                out.append((i, e, e + n))
+        return out
+
+    def chunks_in(self, q, g_lo, g_hi):
+        """The chunk range of slice q whose chunks meet the gradient range [g_lo, g_hi)."""
+        c0, c1 = self.chunk_ranges[q]
+        a = max(c0, bisect.bisect_right(self._starts, g_lo, c0, c1) - 1)
+        b = bisect.bisect_left(self._starts, g_hi, a, c1)
+        return (a, max(a, b))
+
+
+class ShardExchange:
+    """The collectives of a sharded fused optimizer (optim.py shard_state=True), in step order:
+
+      * reduce_scatter(): slice q of G32 on rank q <- the sum over ranks.  Under torch.use_deterministic_algorithms(True) with every
+        rank on this host, GradExchange's phase 1 (rank-ordered, through peer memory) on the plan's bounds.  Otherwise, with NCCL,
+        reduce_scatter_tensor in pieces staged through a fixed buffer (slices padded to the piece length); with gloo, which has no
+        reduce-scatter, an all_gather and the rank-ordered sum (qfx_dp_reduce_det), as GradExchange does on CPU models.
+      * gather_sum(mine, out): the ranks' fp32 partials (one each) all-gathered and added in rank order into out, on the device.
+      * gather_rows(x, rows): x holds this rank's rows [c0, c1) (plan chunk ranges) of a [n_chunks, k] table; the other ranks' rows
+        are all-gathered into it.
+      * gather_weights(): every rank's updated slice of LoRA weights packed (qfx_lora_pack), all-gathered and unpacked into the other
+        ranks' parameter views (qfx_lora_unpack), in pieces of at most STAGING_BYTES.
+    Nothing here waits for the device; all of it is on the current stream."""
+
+    STAGING_BYTES = 64 << 20
+
+    def __init__(self, model, plan: SlicePlan, tables):
+        self.model, self.plan, self.tables = model, plan, tables
+        self.world, self.rank = dist.get_world_size(), dist.get_rank()
+        self.nccl = dist.get_backend() == "nccl"
+        self.dev = model.dev
+        self._stage = None  # STAGING_BYTES, made at the first exchange that needs it
+
+    def _staging(self):
+        if self._stage is None:
+            self._stage = torch.empty(self.STAGING_BYTES, device=self.dev, dtype=torch.uint8)
+        return self._stage
+
+    def reduce_scatter(self):
+        from . import lib
+        g32, (lo, hi) = self.model.G32, self.plan.bounds[self.rank]
+        if torch.are_deterministic_algorithms_enabled():
+            ex = GradExchange.for_model(self.model)
+            if ex is not None:
+                ex.reduce_scatter(self.plan.bounds)
+                return
+        if not self.nccl:
+            bufs = [torch.empty_like(g32) for _ in range(self.world)]
+            dist.all_gather(bufs, g32)
+            if hi > lo:
+                lib.dp_reduce_det([b[lo:hi] for b in bufs], g32[lo:hi])
+            return
+        P = self.STAGING_BYTES // 4 // (self.world + 1)  # fp32 elements per rank and piece: [world, L] sent, [L] received, L <= P
+        stage = self._staging().view(torch.float32)
+        longest = max(b - a for a, b in self.plan.bounds)
+        for k0 in range(0, longest, P):
+            L = min(P, longest - k0)
+            send, recv = stage[: self.world * L].view(self.world, L), stage[self.world * P: self.world * P + L]
+            for r, (a, b) in enumerate(self.plan.bounds):
+                n = max(0, min(L, b - a - k0))
+                send[r, :n] = g32[a + k0: a + k0 + n]
+                send[r, n:] = 0
+            dist.reduce_scatter_tensor(recv, send.view(-1))
+            n = max(0, min(L, hi - lo - k0))
+            g32[lo + k0: lo + k0 + n] = recv[:n]
+
+    def gather_sum(self, mine, out):
+        from . import lib
+        parts = torch.empty(self.world, device=mine.device, dtype=torch.float32)
+        dist.all_gather_into_tensor(parts, mine.reshape(1))
+        lib.dp_reduce_det([parts[r: r + 1] for r in range(self.world)], out.reshape(1))
+
+    def gather_rows(self, x):
+        """x: [n_chunks, k] (any dtype) whose rows of this rank's chunk range are current; afterwards every row is."""
+        rows = [c1 - c0 for c0, c1 in self.plan.chunk_ranges]
+        most = max(rows)
+        if most == 0:
+            return
+        c0, c1 = self.plan.chunk_ranges[self.rank]
+        mine = torch.zeros(most, *x.shape[1:], device=x.device, dtype=x.dtype)
+        mine[: c1 - c0] = x[c0:c1]
+        every = torch.empty(self.world * most, *x.shape[1:], device=x.device, dtype=x.dtype)
+        dist.all_gather_into_tensor(every, mine)
+        for r, (a, b) in enumerate(self.plan.chunk_ranges):
+            if r != self.rank and b > a:
+                x[a:b] = every[r * most: r * most + b - a]
+
+    def gather_weights(self):
+        from . import lib
+        P = self.STAGING_BYTES // 2 // (self.world + 1)  # bf16 elements per rank and piece: [P] packed, [world, P] gathered
+        stage = self._staging().view(torch.bfloat16)
+        send, recv = stage[:P], stage[P: (self.world + 1) * P]
+        plan, q = self.plan, self.rank
+        longest = max(b - a for a, b in plan.bounds)
+        for k0 in range(0, longest, P):
+            L = min(P, longest - k0)
+            lo, hi = plan.bounds[q]
+            a, b = lo + k0, min(hi, lo + k0 + L)
+            if b > a:
+                lib.lora_pack(self.tables, plan.chunks_in(q, a, b), a, b, send[: b - a])
+            dist.all_gather_into_tensor(recv[: self.world * L], send[:L])
+            for r, (lo, hi) in enumerate(plan.bounds):
+                a, b = lo + k0, min(hi, lo + k0 + L)
+                if r != q and b > a:
+                    lib.lora_unpack(self.tables, plan.chunks_in(r, a, b), a, b, recv[r * L: r * L + b - a])
+
+    def gather_ranges(self, x, ranges):
+        """ranges[q] = (a, b): the part of a flat tensor rank q holds, the ranges ascending and covering [0, ranges[-1][1]).  x is this
+        rank's part; returns the whole tensor, assembled on every rank (state_dict)."""
+        most = max(1, max(b - a for a, b in ranges))
+        mine = torch.zeros(most, device=x.device, dtype=x.dtype)
+        mine[: x.numel()] = x.reshape(-1)
+        every = torch.empty(self.world * most, device=x.device, dtype=x.dtype)
+        dist.all_gather_into_tensor(every, mine)
+        return torch.cat([every[r * most: r * most + b - a] for r, (a, b) in enumerate(ranges)])

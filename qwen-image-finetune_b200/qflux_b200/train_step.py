@@ -123,18 +123,20 @@ def _sync_and_step(dit, optimizer, max_grad_norm, micro_steps: int = 1):
     memory of sharding.GradExchange (bit-reproducible), else NCCL's — then either the fused clip + optimizer kernels (FusedLoraAdamW / FusedLoraProdigy / FusedLoraAdam8bit read the
     accumulator directly; every rank then holds the same gradient and parameters, so Prodigy's d and the 8-bit Adam states agree
     across ranks with no further collective) or, for any torch optimizer, mean + clip + cast into the bf16 `.grad` views followed
-    by `optimizer.step()`."""
+    by `optimizer.step()`.  A fused optimizer built with shard_state=True runs the exchange in its own step (reduce-scatter, then the
+    all-gather of the weights), so no all-reduce runs here."""
     from .optim import FusedLoraOptimizer
     from .sharding import GradExchange
+    inner = getattr(optimizer, "optimizer", optimizer)  # accelerate hands the trainer an AcceleratedOptimizer wrapper (.optimizer)
     world = 1
     if dist.is_available() and dist.is_initialized() and dist.get_world_size() > 1:
         world = dist.get_world_size()
-        exchange = GradExchange.for_model(dit) if torch.are_deterministic_algorithms_enabled() else None
-        if exchange is not None:
-            exchange.all_reduce()
-        else:
-            dist.all_reduce(dit.G32)
-    inner = getattr(optimizer, "optimizer", optimizer)  # accelerate hands the trainer an AcceleratedOptimizer wrapper (.optimizer)
+        if not (isinstance(inner, FusedLoraOptimizer) and inner.shard_state):
+            exchange = GradExchange.for_model(dit) if torch.are_deterministic_algorithms_enabled() else None
+            if exchange is not None:
+                exchange.all_reduce()
+            else:
+                dist.all_reduce(dit.G32)
     if isinstance(inner, FusedLoraOptimizer):
         inner.max_grad_norm = max_grad_norm
         inner.grad_divisor = world * micro_steps  # G32 holds the SUM over ranks and micro-steps
