@@ -19,6 +19,7 @@ import warnings
 from typing import NamedTuple
 
 import torch
+import torch.distributed as dist
 import torch.nn as nn
 
 from . import lib
@@ -138,7 +139,7 @@ class FusedMMDiTBase(nn.Module):
     _PER_SINGLE = ()
     _NF4_KINDS = ("mod_w", "qkv_w", "out_w", "up_w", "down_w")  # the stacked matrices a 4-bit base checkpoint keeps NF4-resident
     _SINGLE_MATS: dict = {}     # sub-module name of a single-block Linear -> its stacked kind (FLUX)
-    _sharded_s = None           # sharding.ShardedBlocks of the single blocks once shard_frozen_weights() has run
+    _sharded_s = None           # the single blocks' sharded ring once shard_frozen_weights() has run
 
     def _weight_views(self) -> dict:
         raise NotImplementedError
@@ -192,8 +193,8 @@ class FusedMMDiTBase(nn.Module):
     def _view_source(self, store: bool):
         """(weights dict, whether block entries are included) for `_weight_views`.  store=True: every block, with the NF4- or
         FP8-resident kinds as meta tensors of their bf16 shape — their views' storage offsets address the resident storage
-        (load_state_dict)."""
-        if not store:
+        (load_state_dict).  Sharded weights have no addressable blocks either way."""
+        if not store or self._sharded is not None:
             return self.w, self._blk_rings is None
         w = dict(self.w)
         for k, (codes, _) in self._nf4_store.items():
@@ -230,7 +231,7 @@ class FusedMMDiTBase(nn.Module):
         self._nf4_rings = None   # sharding.Nf4Blocks of (double, single) blocks
         self._fp8_kinds = self._NF4_KINDS if frozen_weights == "fp8" else ()
         self._fp8_store = {}     # FP8-resident kind -> codes float8_e4m3fn [L, ..., out, in]
-        self._expand_rings = None  # sharding.Nf4Blocks / Fp8Blocks of (double, single) blocks: filled from resident storage
+        self._expand_rings = None  # (double, single) rings that expand codes (Nf4Blocks / Fp8Blocks, or their sharded forms)
         self._blk_rings = None   # (double, single) rings the block weights come through: NF4 / FP8 expansion or sharding
         self.dev = torch.device(device)
         self.sites = {}          # (l, grp, s) -> LoraSite   (l = -1: input embedders)
@@ -244,7 +245,8 @@ class FusedMMDiTBase(nn.Module):
         self._rope_cache = {}
         self.gradient_checkpointing = False  # accepted for interface compatibility (see enable_gradient_checkpointing)
         self._activation_limit = None  # bytes the training workspace may take; None: free device memory - ACTIVATION_HEADROOM
-        self._sharded = None     # sharding.ShardedBlocks once shard_frozen_weights() has run (weights sharded across ranks)
+        self._sharded = None     # the double blocks' sharded ring once shard_frozen_weights() has run (weights sharded across ranks):
+                                 # sharding.ShardedBlocks, or ShardedNf4Blocks / ShardedFp8Blocks for NF4 / FP8 codes
         self._grad_exchange = None  # sharding.GradExchange of deterministic data-parallel steps (False: ranks not on one host)
         self._bands_cache = {}   # (valid image rows per sample, Limg) -> lib.RowBands (ragged GEMM row bands)
         self._infer_graphs, self.use_cuda_graph_inference = GraphCache(8, "the inference forward"), True  # see _infer
@@ -305,17 +307,18 @@ class FusedMMDiTBase(nn.Module):
         """BASELINE config 4 (the reference's FSDP branch, base_trainer.py:333-382): keep 1/world of every double and every single
         block's frozen weights on this rank; a block's full weights are assembled in one of two ring buffers right before it runs —
         by copy-engine pulls from the peers' shards on one node, by an NCCL all-gather otherwise (sharding.py; one two-slot ring
-        per block kind).  Call after the weights are loaded.  LoRA factors, embedders and the output head stay replicated;
-        `state_dict()` then only carries the replicated tensors and the LoRA parameters."""
+        per block kind).  Call after the weights are loaded (collective).  LoRA factors, embedders and the output head stay
+        replicated; `state_dict()` then only carries the replicated tensors and the LoRA parameters.
+
+        An NF4- or FP8-resident model (frozen_weights="nf4" / "fp8") shards its codes instead, at world >= 2: each rank keeps 1/world
+        of every block's packed code bytes, and a block is filled by gathering them into a staging slot and expanding them there
+        (sharding.ShardedCodes); biases and norm weights stay replicated bf16.  With the peer gather its steps and inference
+        forwards are still CUDA-graph replayed."""
         from .sharding import ShardedBlocks
         if self._sharded is not None:
             return self
-        if self._nf4_kinds:
-            raise lib.QfxError("shard_frozen_weights: the frozen weights are NF4-resident (frozen_weights='nf4'); sharded NF4 is not "
-                               "supported — shard a bf16 model or train the NF4 model on one GPU per replica")
-        if self._fp8_kinds:
-            raise lib.QfxError("shard_frozen_weights: the frozen weights are FP8-resident (frozen_weights='fp8'); sharded FP8 is not "
-                               "supported — shard a bf16 model or train the FP8 model on one GPU per replica")
+        if self._nf4_kinds or self._fp8_kinds:
+            return self._shard_code_rings(group, gather)
         self._sharded = ShardedBlocks({k: self.w[k] for k in self._PER_LAYER}, self.L, group, gather=gather)
         for k in self._PER_LAYER:
             self.w[k] = self._sharded.rings[k]
@@ -324,6 +327,48 @@ class FusedMMDiTBase(nn.Module):
             for k in self._PER_SINGLE:
                 self.w[k] = self._sharded_s.rings[k]
         self._blk_rings = (self._sharded, self._sharded_s)
+        if torch.cuda.is_available():
+            torch.cuda.empty_cache()
+        return self
+
+    def _shard_code_rings(self, group, gather):
+        """shard_frozen_weights of an NF4- or FP8-resident model: the expansion rings become sharded code rings (one per block kind),
+        and the full code stacks are freed."""
+        from .sharding import ShardedFp8Blocks, ShardedNf4Blocks
+        fmt = "FP8" if self._fp8_kinds else "NF4"
+        world = dist.get_world_size(group) if dist.is_initialized() else 1
+        if world < 2:
+            raise lib.QfxError(f"shard_frozen_weights: the frozen weights are {fmt}-resident (frozen_weights='{fmt.lower()}') and "
+                               f"there is one rank: sharded {fmt} needs world >= 2 (one rank already holds the one copy of the codes)")
+        if self._nf4_kinds and set(self._nf4_kinds) != set(self._NF4_KINDS):
+            raise lib.QfxError(f"shard_frozen_weights: only the stacked kinds {self._nf4_kinds} are NF4-resident (the others bf16); "
+                               f"sharded NF4 needs every stacked block matrix NF4-resident (frozen_weights='nf4')")
+        src = [None if r is None else (r.codes, {k: v.shape for k, v in r.rings.items()}) for r in self._expand_rings]
+        for r in filter(None, self._expand_rings):  # a ring and its views refer to each other: drop its buffers without waiting for gc
+            r.codes = r.gbuf = None
+        self._expand_rings = self._blk_rings = self._nf4_rings = None  # the old slots go back to the allocator before the new ones
+        for _, shapes in filter(None, src):
+            for k in shapes:
+                self.w[k] = None
+        rings = []
+        for ent, n in zip(src, (self.L, self.Ls)):
+            if ent is None:
+                rings.append(None)
+                continue
+            codes, shapes = ent
+            if self._fp8_kinds:
+                ring = ShardedFp8Blocks({k: c for k, (c,) in codes.items()}, n, group, gather=gather)
+            else:
+                ring = ShardedNf4Blocks({k: (c, a, shapes[k]) for k, (c, a) in codes.items()}, n, self.nf4_blocksize, group,
+                                        gather=gather)
+            for k in shapes:
+                self.w[k] = ring.rings[k]
+            rings.append(ring)
+        self._expand_rings = self._blk_rings = tuple(rings)
+        if self._nf4_kinds:
+            self._nf4_rings = self._expand_rings
+        self._sharded, self._sharded_s = rings
+        self._nf4_store, self._fp8_store = {}, {}
         if torch.cuda.is_available():
             torch.cuda.empty_cache()
         return self
@@ -1468,8 +1513,9 @@ class GraphCache:
 
     The first call of a signature runs eagerly (it allocates the workspace, RoPE tables and split-K scratch and sets kernel
     attributes), the second captures `fn` on static copies of the inputs (kernel arguments, TMA descriptors included, are baked in)
-    and every later call copies its inputs into those buffers and replays.  Sharded frozen weights (side-stream all-gathers) and
-    non-CUDA models run eagerly; so does a cache whose capture failed once (with a warning: never silently wrong)."""
+    and every later call copies its inputs into those buffers and replays.  Sharded bf16 frozen weights and shards gathered by NCCL
+    (side-stream all-gathers) and non-CUDA models run eagerly; so does a cache whose capture failed once (with a warning: never
+    silently wrong).  Sharded NF4 / FP8 codes gathered by peer copies are captured (the copies become memcpy nodes)."""
 
     def __init__(self, capacity: int, what: str):
         self.capacity, self.what = capacity, what
@@ -1484,7 +1530,8 @@ class GraphCache:
 
     def run(self, model, fn, args, tag=None, enabled=True):
         """fn(*args) through the graph of key (input signature, tag)."""
-        if not enabled or self.failed or model._sharded is not None or model.dev.type != "cuda" or not torch.cuda.is_available():
+        sharded = model._sharded is not None and not getattr(model._sharded, "capturable", False)
+        if not enabled or self.failed or sharded or model.dev.type != "cuda" or not torch.cuda.is_available():
             return fn(*args)
         key = (_graph_sig(args), tag, torch.are_deterministic_algorithms_enabled())  # never replay across the two kernel choices
         ent = self.entries.pop(key, None)

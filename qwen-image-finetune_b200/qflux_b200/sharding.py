@@ -17,9 +17,11 @@ parallel mode.  B200-first layout instead of FSDP's per-module flat parameters:
     for another.  `gather="nccl"` (or QFX_SHARD_GATHER=nccl, or ranks on different hosts) keeps the all_gather_into_tensor path;
   * kernels keep reading plain row-major [out, in] views — the views now point into the gather buffer of the block's slot.
 
-The same two-slot ring (`BlockRing`) has two more fill sources: `Nf4Blocks` dequantizes a block's NF4-resident matrices
+The same two-slot ring (`BlockRing`) has more fill sources: `Nf4Blocks` dequantizes a block's NF4-resident matrices
 (4-bit base checkpoints, nf4.py) into its slot with one kernel launch, and `Fp8Blocks` expands its FP8-resident matrices
-(float8-e4m3fn base checkpoints, fp8.py) the same way.
+(float8-e4m3fn base checkpoints, fp8.py) the same way.  `ShardedNf4Blocks` / `ShardedFp8Blocks` shard those codes across the
+ranks: a block's code bytes are gathered as above (`ShardGather`, shared with `ShardedBlocks`) into a staging slot, then expanded
+from there by the same launch.
 """
 from __future__ import annotations
 
@@ -31,6 +33,7 @@ import torch
 import torch.distributed as dist
 
 ALIGN = 128  # elements (256 B): every packed tensor starts on a TMA-friendly boundary
+ALIGN_BYTES = 2 * ALIGN  # the same boundary for rows of any element type (sharded rows are padded to it per rank)
 
 
 class LayerRing:
@@ -132,53 +135,58 @@ class BlockRing:
                 e.record(torch.cuda.current_stream())
 
 
-class ShardedBlocks(BlockRing):
-    def __init__(self, stacked: dict, n_layers: int, group=None, gather: str = "auto"):
-        """stacked: {name: tensor [L, ...]} (full copies; released by the caller afterwards).
-        gather: "auto" (peer copies when every rank is a CUDA device of this host, else NCCL), "peer", or "nccl"."""
+class ShardGather:
+    """The gather half of a sharded ring: this rank keeps columns [rank n_shard, (rank + 1) n_shard) of a layer-stacked [L, n_blk]
+    matrix whose rows are the packed blocks, and `_pull(dst, l)` assembles row l into dst on the current stream.  On one host every
+    rank exports its shard once through CUDA IPC and a row is `world` copy-engine pulls from the mapped peer pointers, starting at the
+    next rank; otherwise (or with gather="nccl") it is one all_gather_into_tensor.  Used by ShardedBlocks (bf16 rows) and by
+    ShardedNf4Blocks / ShardedFp8Blocks (rows of NF4 / FP8 code bytes)."""
+
+    def _init_shards(self, parts, n_row: int, n_layers: int, dtype, group, gather: str):
+        """parts: [(offset in the row, tensor [L, n] of `dtype`)], the row segments (full copies; released by the caller afterwards).
+        The row is padded to whole ALIGN_BYTES per rank.  gather: "auto" (peer copies when every rank is a CUDA device of this host,
+        else NCCL), "peer", or "nccl".  Collective."""
         self.group = group
         self.world = dist.get_world_size(group) if dist.is_initialized() else 1
         self.rank = dist.get_rank(group) if dist.is_initialized() else 0
-        any_t = next(iter(stacked.values()))
-        for t in stacked.values():
-            assert t.shape[0] == n_layers
-        off = self._layout({name: t.shape[1:] for name, t in stacked.items()}, n_layers, any_t.device, any_t.dtype)
-        q = self.world * ALIGN
-        self.n_blk = -(-off // q) * q
+        q = self.world * (ALIGN_BYTES // dtype.itemsize)
+        self.n_blk = -(-n_row // q) * q
         self.n_shard = self.n_blk // self.world
         self.gather = self._pick_gather(os.environ.get("QFX_SHARD_GATHER", gather))
         self._peer_buf, self._peer_ptrs = None, None
         if self.gather == "peer":
             from . import lib
-            self._peer_buf = lib.PeerBuffer(n_layers * self.n_shard * self.dtype.itemsize, self.dev)
-            self.shard = self._peer_buf.tensor(self.dtype, (n_layers, self.n_shard))
+            self._peer_buf = lib.PeerBuffer(n_layers * self.n_shard * dtype.itemsize, self.dev)
+            self.shard = self._peer_buf.tensor(dtype, (n_layers, self.n_shard))
             self.shard.zero_()
         else:
-            self.shard = torch.zeros(n_layers, self.n_shard, device=self.dev, dtype=self.dtype)
+            self.shard = torch.zeros(n_layers, self.n_shard, device=self.dev, dtype=dtype)
         lo, hi = self.rank * self.n_shard, (self.rank + 1) * self.n_shard
-        for name, t in stacked.items():
-            r = self.rings[name]
-            a, b = max(lo, r.offset), min(hi, r.offset + r.numel)
+        for off, t in parts:
+            a, b = max(lo, off), min(hi, off + t.shape[1])
             if a < b:
-                self.shard[:, a - lo: b - lo] = t.reshape(n_layers, -1)[:, a - r.offset: b - r.offset]
-        self._alloc_slots(self.n_blk)
+                self.shard[:, a - lo: b - lo] = t[:, a - off: b - off]
         if self.gather == "peer":
             self._open_peers()
 
-    def _fill(self, s: int, l: int):
+    @property
+    def capturable(self) -> bool:
+        """Whether a forward through this ring may be captured into a CUDA graph (GraphCache)."""
+        return False
+
+    def _pull(self, dst, l: int):
+        """dst (the [n_blk] row buffer) <- row l, assembled from every rank's shard on the current stream."""
         if self.world == 1:
-            self.gbuf[s].copy_(self.shard[l])
+            dst.copy_(self.shard[l])
         elif self.gather == "peer":
             from . import lib
-            nb = self.n_shard * self.dtype.itemsize
-            dst = self.gbuf[s].data_ptr()
+            nb = self.n_shard * self.shard.element_size()
             for i in range(self.world):  # own shard last; the pulls start at the next rank so no port sees all ranks at once
                 r = (self.rank + 1 + i) % self.world
-                lib.peer_copy_async(dst + r * nb, self._peer_ptrs[r] + l * nb, nb)
+                lib.peer_copy_async(dst.data_ptr() + r * nb, self._peer_ptrs[r] + l * nb, nb)
         else:
-            dist.all_gather_into_tensor(self.gbuf[s], self.shard[l], group=self.group)
+            dist.all_gather_into_tensor(dst, self.shard[l], group=self.group)
 
-    # ------------------------------------------------------------------------------------------------------------
     def _pick_gather(self, want: str) -> str:
         if want not in ("auto", "peer", "nccl"):
             raise ValueError(f"gather must be auto|peer|nccl, got {want!r}")
@@ -218,6 +226,22 @@ class ShardedBlocks(BlockRing):
             dist.barrier(group=self.group)
             self.shard = None
             self._peer_buf.free()
+
+
+class ShardedBlocks(ShardGather, BlockRing):
+    def __init__(self, stacked: dict, n_layers: int, group=None, gather: str = "auto"):
+        """stacked: {name: tensor [L, ...]} (full copies; released by the caller afterwards).
+        gather: "auto" (peer copies when every rank is a CUDA device of this host, else NCCL), "peer", or "nccl"."""
+        any_t = next(iter(stacked.values()))
+        for t in stacked.values():
+            assert t.shape[0] == n_layers
+        off = self._layout({name: t.shape[1:] for name, t in stacked.items()}, n_layers, any_t.device, any_t.dtype)
+        self._init_shards([(self.rings[name].offset, t.reshape(n_layers, -1)) for name, t in stacked.items()], off, n_layers,
+                          self.dtype, group, gather)
+        self._alloc_slots(self.n_blk)
+
+    def _fill(self, s: int, l: int):
+        self._pull(self.gbuf[s], l)
 
 
 class GradExchange:
@@ -350,7 +374,26 @@ class GradExchange:
             self._buf = None
 
 
-class Nf4Blocks(BlockRing):
+class CodeBlocks(BlockRing):
+    """A ring filled by expanding a block's resident codes: `codes` holds {kind: (layer-stacked code tensors [L, ...] of one matrix)},
+    and `_expand(s, src)` fills slot s from {kind: (the flat code tensors of one layer)} in ONE launch (the segment table).  The
+    sources are the resident stacks here, a staging slot of gathered shards in ShardedCodes."""
+
+    def _layer_codes(self, l: int) -> dict:
+        return {k: tuple(t[l].reshape(-1) for t in ts) for k, ts in self.codes.items()}
+
+    def _out(self, s: int, k: str):
+        r = self.rings[k]
+        return self.gbuf[s, r.offset: r.offset + r.numel]
+
+    def _expand(self, s: int, src: dict):
+        raise NotImplementedError
+
+    def _fill(self, s: int, l: int):
+        self._expand(s, self._layer_codes(l))
+
+
+class Nf4Blocks(CodeBlocks):
     """NF4-resident frozen weights: every NF4 matrix of a block kind lives as layer-stacked codes + fp32 absmax (nf4.py); a block's
     bf16 matrices are produced in its ring slot by ONE qfx_nf4_dequant launch right before it runs.  Kernels read the same
     row-major [out, in] bf16 views as for resident or sharded weights."""
@@ -359,16 +402,15 @@ class Nf4Blocks(BlockRing):
         """stacks: {name: (codes uint8 [L, ..., in/2], absmax fp32 [L, n/blocksize], bf16 shape of one layer)}."""
         codes0 = next(iter(stacks.values()))[0]
         off = self._layout({k: shape for k, (_, _, shape) in stacks.items()}, n_layers, codes0.device, torch.bfloat16)
-        self.stacks, self.blocksize = stacks, blocksize
+        self.codes, self.blocksize = {k: (c, a) for k, (c, a, _) in stacks.items()}, blocksize
         self._alloc_slots(off)
 
-    def _fill(self, s: int, l: int):
+    def _expand(self, s: int, src: dict):
         from . import lib
-        lib.nf4_dequant([(c[l].reshape(-1), a[l].reshape(-1), self.gbuf[s, self.rings[k].offset: self.rings[k].offset + self.rings[k].numel],
-                          self.blocksize) for k, (c, a, _) in self.stacks.items()])
+        lib.nf4_dequant([(c, a, self._out(s, k), self.blocksize) for k, (c, a) in src.items()])
 
 
-class Fp8Blocks(BlockRing):
+class Fp8Blocks(CodeBlocks):
     """FP8-resident frozen weights: every FP8 matrix of a block kind lives as layer-stacked float8-e4m3fn codes (fp8.py), one byte
     per element in the bf16 layout; a block's bf16 matrices are produced in its ring slot by ONE qfx_fp8_expand launch right before
     it runs (exact: every finite e4m3fn value is a bf16 value)."""
@@ -377,13 +419,61 @@ class Fp8Blocks(BlockRing):
         """stacks: {name: codes float8_e4m3fn [L, ...] (the bf16 shape of the stack)}."""
         codes0 = next(iter(stacks.values()))
         off = self._layout({k: tuple(c.shape[1:]) for k, c in stacks.items()}, n_layers, codes0.device, torch.bfloat16)
-        self.stacks = stacks
+        self.codes = {k: (c,) for k, c in stacks.items()}
         self._alloc_slots(off)
 
-    def _fill(self, s: int, l: int):
+    def _expand(self, s: int, src: dict):
         from . import lib
-        lib.fp8_expand([(c[l].reshape(-1), self.gbuf[s, self.rings[k].offset: self.rings[k].offset + self.rings[k].numel])
-                        for k, c in self.stacks.items()])
+        lib.fp8_expand([(c, self._out(s, k)) for k, (c,) in src.items()])
+
+
+class ShardedCodes(ShardGather):
+    """Sharded NF4 / FP8 frozen weights: the resident codes of one block (every NF4 matrix's uint8 codes and fp32 absmax, or every
+    FP8 matrix's e4m3fn bytes) are packed into ONE byte row, each tensor on an ALIGN_BYTES boundary, and this rank keeps 1/world of
+    every layer's row (ShardGather).  A block is filled in two stages on the ring's side stream: the W shards of its row are gathered
+    into a per-slot staging buffer, then ONE expansion launch (the subclass's `_expand`, the same segment table as for resident codes)
+    runs from the staging slot into the bf16 slot.  Both stages are ordered by the ring's prefetch / acquire / release events, so the
+    block kernels read the same bf16 views as for resident codes; the peer pulls are copies, so a forward through the ring can be
+    captured into a CUDA graph (memcpy nodes), the NCCL all-gather cannot."""
+
+    def _shard_codes(self, group, gather):
+        """Replace `codes` by this rank's shard of the packed rows and allocate the two staging slots (collective)."""
+        row, parts, off = {}, [], 0
+        for k, ts in self.codes.items():
+            row[k] = []
+            for t in ts:
+                flat = t.reshape(self.L, -1)
+                row[k].append((off, flat.shape[1], t.dtype))
+                parts.append((off, flat.view(torch.uint8)))
+                off += -(-flat.shape[1] * t.element_size() // ALIGN_BYTES) * ALIGN_BYTES
+        self._init_shards(parts, off, self.L, torch.uint8, group, gather)
+        self.codes = None  # the full stacks are the caller's to free
+        self.stage = torch.zeros(2, self.n_blk, device=self.dev, dtype=torch.uint8)
+        # the segment tables' sources: every code tensor of a block as a view into each staging slot
+        self._staged = [{k: tuple(self.stage[s, o: o + n * dt.itemsize].view(dt) for o, n, dt in segs) for k, segs in row.items()}
+                        for s in range(2)]
+
+    @property
+    def capturable(self) -> bool:
+        return self.gather == "peer"
+
+    def _fill(self, s: int, l: int):
+        self._pull(self.stage[s], l)
+        self._expand(s, self._staged[s])
+
+
+class ShardedNf4Blocks(ShardedCodes, Nf4Blocks):
+    def __init__(self, stacks: dict, n_layers: int, blocksize: int, group=None, gather: str = "auto"):
+        """stacks: as for Nf4Blocks (full copies; released by the caller afterwards); group / gather: as for ShardedBlocks."""
+        Nf4Blocks.__init__(self, stacks, n_layers, blocksize)
+        self._shard_codes(group, gather)
+
+
+class ShardedFp8Blocks(ShardedCodes, Fp8Blocks):
+    def __init__(self, stacks: dict, n_layers: int, group=None, gather: str = "auto"):
+        """stacks: as for Fp8Blocks (full copies; released by the caller afterwards); group / gather: as for ShardedBlocks."""
+        Fp8Blocks.__init__(self, stacks, n_layers)
+        self._shard_codes(group, gather)
 
 
 class SlicePlan:
