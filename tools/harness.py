@@ -35,7 +35,7 @@ def time_cuda(fn, iters=20, warmup=3, flush=None):
     return ts[len(ts) // 2]
 
 
-def main(cases: dict, script: str, out_name: str):
+def main(cases: dict, script: str, out_name: str, timeout: float = 300):
     if len(sys.argv) >= 3 and sys.argv[1] == "--case":
         res = cases[sys.argv[2]]()
         print("RESULT " + json.dumps(res))
@@ -47,7 +47,7 @@ def main(cases: dict, script: str, out_name: str):
     for name in only:
         t0 = time.time()
         try:
-            r = subprocess.run([sys.executable, script, "--case", name], capture_output=True, text=True, timeout=300)
+            r = subprocess.run([sys.executable, script, "--case", name], capture_output=True, text=True, timeout=timeout)
             out = r.stdout + r.stderr
             res = [l for l in r.stdout.splitlines() if l.startswith("RESULT ")]
             status = "ok" if (r.returncode == 0 and res) else f"FAIL rc={r.returncode}"
