@@ -17,6 +17,10 @@
 
 Each case returns a dict of measurements plus `fail`, the list of violated checks (each names its problem, tile or row).  Run
 stand-alone: `python tools/gemm_tile_check.py [case ...]` (one subprocess per case).
+
+Every launch here has fewer tiles than an H100 has SMs, so each CTA of the persistent kernel computes exactly one tile.  What
+happens between a CTA's tiles (the ring carried over, the next tile's problem and k-block count, the epilogue overlapped with the
+next tile's loads) is checked by tools/gemm_sched_check.py, which runs `run` on launches with several tiles per CTA.
 """
 import os
 import sys
@@ -187,8 +191,9 @@ def _tile_of(M, bands, device):
     return t, live
 
 
-def _regions(c, name, k, e, ref, tile_of, bn, live=None):
-    """relative L2 of kernel and bf16 eager against fp64 per (m-tile, n-tile) and per row: err_k <= C * err_e + FLOOR"""
+def _regions(c, name, k, e, ref, tile_of, bn, live=None, rows=True):
+    """relative L2 of kernel and bf16 eager against fp64 per (m-tile, n-tile) and per row: err_k <= C * err_e + FLOOR (per row only
+    when `rows`; the ratio is reported either way)"""
     if live is not None:
         k, e, ref, tile_of = k[live], e[live], ref[live], tile_of[live]
     ref = ref.double()
@@ -211,7 +216,7 @@ def _regions(c, name, k, e, ref, tile_of, bn, live=None):
     for mt, n_t in bad.nonzero().tolist()[:3]:
         c.fail.append(f"{name} tile (m{mt}, n{n_t}): kernel {tk[mt, n_t].item():.3e} vs bf16 eager {te[mt, n_t].item():.3e}")
     row_id = torch.arange(M, device=ref.device) if live is None else live.nonzero().flatten()
-    for i in (~(rk <= C_ROW * re_ + FLOOR_ROW)).nonzero().flatten().tolist()[:3]:
+    for i in (~(rk <= C_ROW * re_ + FLOOR_ROW)).nonzero().flatten().tolist()[:3] if rows else []:
         c.fail.append(f"{name} row {int(row_id[i])}: kernel {rk[i].item():.3e} vs bf16 eager {re_[i].item():.3e}")
 
 
@@ -242,9 +247,10 @@ def _ulp_bound(c, name, k, want64, fp32_err):
         c.fail.append(f"{name}: {int((~ok).sum())} elements beyond one ulp of the rule, first rows {r[:4].tolist()}")
 
 
-def run(c, tag, probs, N, K, *, trans_b, epi, alpha=1.0, bn, lora_group_n=0, attn=None, emu_check=True, alias=False):
+def run(c, tag, probs, N, K, *, trans_b, epi, alpha=1.0, bn, lora_group_n=0, attn=None, emu_check=True, alias=False, rows=True):
     """probs: list of dicts of device tensors (A, B, optional A2/B2/kb2/a2_col0, bias, resid, gate/rows_per_batch, aux, with_out2,
-    bands, s_offset).  attn (ATTN_DO): dict(B, H, S).  alias (ADD): out is the resid buffer itself."""
+    bands, s_offset).  attn (ATTN_DO): dict(B, H, S).  alias (ADD): out is the resid buffer itself.  rows: hold every row to the
+    per-row bound (see gemm_sched_check.py for launches whose rows are too short for it)."""
     from qflux_b200 import lib
     dev = probs[0]["A"].device
     full, lp = [], []
@@ -306,7 +312,7 @@ def run(c, tag, probs, N, K, *, trans_b, epi, alpha=1.0, bn, lora_group_n=0, att
         for o in got:
             if o == "delta":
                 continue
-            _regions(c, f"{pn}_{o}", got[o], eag[o], ref[o], tile_of, bn, live)
+            _regions(c, f"{pn}_{o}", got[o], eag[o], ref[o], tile_of, bn, live, rows)
         # (b) the stated rounding rule on the kernel's own accumulator
         if epi != EPI_BIAS:
             want = rule(pr, rbs[i], epi)
