@@ -94,8 +94,8 @@ int qfx_zero_rows(void* out, int64_t ld, int ncols, const int* ranges, int n_ran
  * >= kv_len[b]; txt_len (int32 [B], may be NULL) additionally masks the text padding, keys in [txt_len[b], split).
  * Forward writes O token-major into two row groups: rows with joint position s < split of sample b go to
  * out0[(b*rows0 + s)*ld0 + h*128 ..], the others to out1[(b*rows1 + s - split)*ld1 + h*128 ..]; lse is the log2-domain
- * log-sum-exp [B,H,S].  Backward: dQ_accum is fp32 [B,H,S,128], zeroed by the caller (every key tile adds into it);
- * delta = rowsum(dO * O) [B,H,S].  txt_len needs 0 < split <= S.  Forward: rows0 >= split, rows1 >= S - split, out0 / out1
+ * log-sum-exp [B,H,S].  Backward: dQ_accum is fp32 [B,H,S,128], zeroed by the caller (every key tile adds into it), 16-byte
+ * aligned for qfx_attn_bwd (it is reduced into through a tensor map), 8-byte for qfx_attn_bwd_det; delta = rowsum(dO * O) [B,H,S].  txt_len needs 0 < split <= S.  Forward: rows0 >= split, rows1 >= S - split, out0 / out1
  * 16-byte aligned with ld0 / ld1 >= H*128 and multiples of 8.  A query tile of only padding rows (every position >= kv_len[b]
  * and >= split) gets O = 0 and lse = 0. */
 int qfx_attn_fwd(const void* Q, const void* K, const void* V, void* out0, int64_t ld0, int rows0, void* out1, int64_t ld1,

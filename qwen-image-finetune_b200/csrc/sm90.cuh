@@ -70,6 +70,21 @@ __device__ __forceinline__ void tma_load_3d(uint32_t dst, const CUtensorMap* m, 
       ::"r"(dst), "l"(m), "r"(bar), "r"(c0), "r"(c1), "r"(c2)
       : "memory");
 }
+// Element-wise fp32 add of a shared-memory box into global memory (rows outside the tensor map are clipped).  The generic-proxy
+// stores that filled the box must be made visible first (fence_proxy_async_smem); the issuing thread commits the op to a bulk
+// group and waits on it (tma_store_wait_read) before the box is written again, and (tma_store_wait) before the CTA exits.
+__device__ __forceinline__ void tma_reduce_add_3d(const CUtensorMap* m, uint32_t src, int c0, int c1, int c2) {
+  asm volatile("cp.reduce.async.bulk.tensor.3d.global.shared::cta.add.tile.bulk_group [%0, {%2, %3, %4}], [%1];"
+               ::"l"(m), "r"(src), "r"(c0), "r"(c1), "r"(c2)
+               : "memory");
+}
+__device__ __forceinline__ void tma_store_commit() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
+// the shared-memory sources of every committed group but the newest N have been read
+template <int N>
+__device__ __forceinline__ void tma_store_wait_read() { asm volatile("cp.async.bulk.wait_group.read %0;" ::"n"(N) : "memory"); }
+// every committed group but the newest N has completed
+template <int N>
+__device__ __forceinline__ void tma_store_wait() { asm volatile("cp.async.bulk.wait_group %0;" ::"n"(N) : "memory"); }
 // ------------------------------------------------------------------------------------------------ wgmma (sm_90a)
 // Shared-memory matrix descriptor (64 bit):
 //   [0,14)  start address >> 4        [16,30) leading-dim byte offset >> 4     [32,46) stride-dim byte offset >> 4
